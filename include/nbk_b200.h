@@ -144,6 +144,25 @@ int nbk_r2c(const void *real, void *cplx, int dtype, const int64_t *nmesh_host, 
 int nbk_c2r(const void *cplx, void *real, int dtype, const int64_t *nmesh_host, void *work,
             void *stream);
 
+/* Mixed-radix transforms for sides that are products of 2, 3, 5 and 7 (pmesh/pfft accept any size; nbodykit scripts use
+ * meshes like 96, 100, 360, 768, 1536): the same RealField.r2c / ComplexField.c2r (base/mesh.py:228,237;
+ * source/mesh/catalog.py:341-351) with the semantics of nbk_r2c / nbk_c2r -- forward normalised by 1/(Nx*Ny*Nz) times
+ * extra_scale (folded into the last pass), backward unnormalised, c2r preserves its input when `work` is given.
+ * Limits: Nx, Ny in 2 .. 4096; Nz in 2 .. 8192 if even, up to 4095 if odd (every complex line <= 4096 points).
+ * Powers of two are accepted as well. */
+int nbk_r2c_mixed(const void *real, void *cplx, int dtype, const int64_t *nmesh_host, double extra_scale, void *stream);
+int nbk_c2r_mixed(const void *cplx, void *real, int dtype, const int64_t *nmesh_host, void *work, void *stream);
+/* the passes of the mixed-radix transform, for the slab-decomposed route (P > 1, base/mesh.py:228,237):
+ *   lines : complex FFT of length n_line (2 .. 4096, 7-smooth) along element(outer, n, inner) =
+ *           data[outer*outer_stride + n*line_stride + inner], inner < n_inner; out = scale * DFT (inverse != 0: the
+ *           unnormalised inverse DFT times scale).  src == dst: in place.
+ *   z     : real rows [rows][Nz] -> complex rows [rows][Nz/2+1] (inverse == 0), or back (inverse != 0, unnormalised);
+ *           the output is multiplied by scale. */
+int nbk_fft_lines_mixed(const void *src, void *dst, int dtype, int64_t n_line, int64_t line_stride, int64_t n_inner,
+                        int64_t n_outer, int64_t outer_stride, int inverse, double scale, void *stream);
+int nbk_fft_z_mixed(const void *in, void *out, int dtype, int64_t rows, int64_t Nz, int inverse, double scale,
+                    void *stream);
+
 /* the three 1-D passes of the slab-decomposed transform, for the multi-GPU path (P > 1):
  *   zy pass : real slab [x_n][Ny][Nz] -> cplx slab [x_n][Ny][Nzc], r2c along z then FFT along y
  *   pack    : cplx slab [x_n][Ny][Nzc] -> send buffer [P][y_n][x_n][Nzc] (block p = y rows of rank p)

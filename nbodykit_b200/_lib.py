@@ -44,6 +44,10 @@ SIGNATURES = {
     "nbk_sum_w_w2": ([_vp, _i, _i64, _vp, _vp], _i),
     "nbk_r2c": ([_vp, _vp, _i, _pi64, _d, _vp], _i),
     "nbk_c2r": ([_vp, _vp, _i, _pi64, _vp, _vp], _i),
+    "nbk_r2c_mixed": ([_vp, _vp, _i, _pi64, _d, _vp], _i),
+    "nbk_c2r_mixed": ([_vp, _vp, _i, _pi64, _vp, _vp], _i),
+    "nbk_fft_lines_mixed": ([_vp, _vp, _i, _i64, _i64, _i64, _i64, _i64, _i, _d, _vp], _i),
+    "nbk_fft_z_mixed": ([_vp, _vp, _i, _i64, _i64, _i, _d, _vp], _i),
     "nbk_fft_zy_forward": ([_vp, _vp, _i, _i64, _i64, _i64, _vp], _i),
     "nbk_fft_zy_backward": ([_vp, _vp, _i, _i64, _i64, _i64, _vp], _i),
     "nbk_fft_lines": ([_vp, _i, _i64, _i64, _i64, _i64, _i64, _i, _d, _vp], _i),

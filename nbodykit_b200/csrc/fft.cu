@@ -16,6 +16,8 @@
 // shared-memory kernels (k_fft_lines with cp.async double buffering, k_fft_z_r2c, k_fft_z_c2r).
 // Decimation-in-frequency radix-8 butterflies in registers throughout (+ one radix-4 / radix-2 stage for the remainder of
 // log2 N).  Twiddles: f8-accurate table built on the device with sincospi, staged in shared memory.  Sizes: 2^k.
+// Sides that are products of 2, 3, 5 and 7 (Nx, Ny <= 4096; Nz <= 8192 even, <= 4095 odd) go through the separate
+// mixed-radix entry points at the end of this file (k_fft_lines_mixed, k_fft_z_mixed; nbk_r2c_mixed / nbk_c2r_mixed).
 #include "common.cuh"
 #include <cuda.h>      // CUtensorMap types only: the encoder comes from cudaGetDriverEntryPoint (no -lcuda)
 #include <map>
@@ -1841,8 +1843,10 @@ k_hermitian_compress(const C *__restrict__ full, C *__restrict__ comp, int64_t r
 }
 
 extern "C" int nbk_hermitian_expand(const void *comp, void *full, int dtype, const int64_t *nmesh, void *stream) {
-    int rc = check_dims("hermitian_expand", dtype, nmesh[0], nmesh[1], nmesh[2]);
-    if (rc) return rc;
+    NBK_CHECK_ARG(dtype == NBK_F4 || dtype == NBK_F8, "hermitian_expand: bad dtype %d", dtype);
+    NBK_CHECK_ARG(nmesh[0] >= 2 && nmesh[1] >= 2 && nmesh[2] >= 2 && nmesh[0] < (1 << 24) && nmesh[1] < (1 << 24) &&
+                  nmesh[2] < (1 << 24), "hermitian_expand: Nmesh (%lld,%lld,%lld) unsupported: sides must be >= 2",
+                  (long long)nmesh[0], (long long)nmesh[1], (long long)nmesh[2]);
     NBK_CHECK_ARG(comp != nullptr && full != nullptr && comp != full, "hermitian_expand: needs two distinct buffers");
     int64_t rows = nmesh[0] * nmesh[1];
     int g = nbk_grid_for(rows * 32, 256, 8);
@@ -1996,4 +2000,514 @@ extern "C" int nbk_slab_push(const void *send, void *const *peer_ptrs_host, int 
         NBK_CUDA(cudaMemcpy2DAsync(dstp, dpitch, srcp, width, width, (size_t)rows_per_peer, cudaMemcpyDeviceToDevice, s));
     }
     return NBK_OK;
+}
+
+// =============================================================================================
+// Mixed-radix path: sides N = 2^a 3^b 5^c 7^d (pmesh / pfft accept any size; nbodykit scripts use 96, 100, 360, 768,
+// 1536 ...).  Separate entry points (nbk_r2c_mixed, nbk_c2r_mixed, nbk_fft_lines_mixed, nbk_fft_z_mixed): the
+// power-of-two kernels above are untouched.
+//   plan     : in-place decimation in frequency over a host-chosen list of radices from {8, 4, 2, 7, 5, 3} (radix 8 while
+//              three factors of two remain, then one 4 or 2, then the odd factors), packed 4 bits per stage into one
+//              kernel argument.  One register butterfly per radix; 3, 5 and 7 use constant roots.  The output position
+//              of frequency k is the mixed-radix digit reversal of k for that plan, tabulated once per CTA in shared
+//              memory (ushort[N]).
+//   inverse  : IDFT(x)[k] = DFT(x)[(N - k) mod N] -- the store reads the reversed frequency, nothing is conjugated.
+//   lines    : k_fft_lines_mixed, the k_fft_lines skeleton (tiles [N][B+1] of B adjacent columns, cp.async double
+//              buffering, twiddles W_N^i staged in shared memory, scale folded into the store).
+//   z pass   : k_fft_z_mixed, a tile of whole contiguous rows per CTA (lanes along the row).  Even Nz: packed
+//              Nz/2-point complex FFT + Hermitian split with W_Nz^k (the inverse combines first).  Odd Nz: two real rows
+//              packed as re + i im, one Nz-point FFT, X_a = (Z[k] + conj Z[-k]) / 2, X_b = (Z[k] - conj Z[-k]) / 2i; the
+//              inverse rebuilds both Hermitian rows in shared memory while loading.
+//   limits   : every complex line is at most 4096 points (Nx, Ny <= 4096; even Nz <= 8192; odd Nz <= 4095): every tile,
+//              twiddle table and digit-reversal table then fits in 227 KB of shared memory.
+// =============================================================================================
+#define NBK_MR_MAX_LINE 4096
+#define NBK_MR_MAX_STAGES 16
+
+struct MixedPlan {
+    int n;                        // complex points per line
+    int nstage;
+    unsigned long long radices;   // radix of stage s in bits [4 s, 4 s + 4); stage 0 splits the whole line
+};
+
+__device__ __forceinline__ int mr_radix(const MixedPlan &p, int s) { return (int)((p.radices >> (4 * s)) & 15); }
+
+// cos / sin (2 pi h / R) of the odd radices, 1 <= h < R (constant-folded once the butterfly loops are unrolled)
+__device__ __forceinline__ double mr_cos(int R, int h) {
+    if (h > R / 2) h = R - h;
+    if (R == 3) return -0.5;
+    if (R == 5) return h == 1 ? 0.30901699437494742410 : -0.80901699437494742410;
+    return h == 1 ? 0.62348980185873353053 : (h == 2 ? -0.22252093395631440429 : -0.90096886790241912624);
+}
+__device__ __forceinline__ double mr_sin(int R, int h) {
+    const double sg = h > R / 2 ? -1.0 : 1.0;
+    if (h > R / 2) h = R - h;
+    if (R == 3) return sg * 0.86602540378443864676;
+    if (R == 5) return sg * (h == 1 ? 0.95105651629515357212 : 0.58778525229247312917);
+    return sg * (h == 1 ? 0.78183148246802980871 : (h == 2 ? 0.97492791218182360702 : 0.43388373911755812048));
+}
+
+// R-point forward DFT, R odd, natural order in and out:  X_m = A_m - i B_m,  X_{R-m} = A_m + i B_m  with
+// A_m = a_0 + sum_j cos(2 pi j m / R) (a_j + a_{R-j}),  B_m = sum_j sin(2 pi j m / R) (a_j - a_{R-j}),  j = 1 .. (R-1)/2
+template <typename T, typename C, int R>
+__device__ __forceinline__ void dft_odd(C (&a)[R]) {
+    constexpr int H = (R - 1) / 2;
+    C s[H], d[H];
+    C x0 = a[0];
+#pragma unroll
+    for (int j = 1; j <= H; j++) {
+        s[j - 1] = cadd(a[j], a[R - j]);
+        d[j - 1] = csub(a[j], a[R - j]);
+        x0 = cadd(x0, s[j - 1]);
+    }
+#pragma unroll
+    for (int m = 1; m <= H; m++) {
+        C A = a[0], Bm = C{0, 0};
+#pragma unroll
+        for (int j = 1; j <= H; j++) {
+            const T c = (T)mr_cos(R, (j * m) % R), sn = (T)mr_sin(R, (j * m) % R);
+            A.x += c * s[j - 1].x;
+            A.y += c * s[j - 1].y;
+            Bm.x += sn * d[j - 1].x;
+            Bm.y += sn * d[j - 1].y;
+        }
+        a[m] = C{A.x + Bm.y, A.y - Bm.x};
+        a[R - m] = C{A.x - Bm.y, A.y + Bm.x};
+    }
+    a[0] = x0;
+}
+
+template <typename T, typename C, int R>
+__device__ __forceinline__ void dft_mixed(C (&a)[R]) {
+    if constexpr (R == 8) radix8(a);
+    else if constexpr (R == 4) dft4(a[0], a[1], a[2], a[3]);
+    else if constexpr (R == 2) { C x0 = a[0], x1 = a[1]; a[0] = cadd(x0, x1); a[1] = csub(x0, x1); }
+    else dft_odd<T, C, R>(a);
+}
+
+// tile row pitch: B + 1 elements (conflict-free quarter-warp accesses); a single column needs no padding
+template <int B> struct MrPitch { static constexpr int v = B > 1 ? B + 1 : 1; };
+
+// one DIF stage of radix R over B side-by-side lines: sub-transforms of length Ns, Q = Ns / R.  Twiddle
+// W_Ns^{q m} = tw[q m (N / Ns) twmul]  (tw is W_{N twmul}^i: twmul = 2 when the table belongs to the unpacked row)
+template <typename T, typename C, int B, int R>
+__device__ __forceinline__ void mr_stage(C *sm, const C *tw, int N, int Ns, int twmul) {
+    constexpr int pitch = MrPitch<B>::v;
+    const int Q = Ns / R;
+    const int tws = (N / Ns) * twmul;
+    const int work = (N / R) * B;
+    for (int w = threadIdx.x; w < work; w += blockDim.x) {
+        const int b = w % B, t = w / B;
+        const int blk = t / Q, q = t - blk * Q;
+        C *p = sm + (blk * Ns + q) * pitch + b;
+        C a[R];
+#pragma unroll
+        for (int j = 0; j < R; j++) a[j] = p[j * Q * pitch];
+        dft_mixed<T, C, R>(a);
+        p[0] = a[0];
+        const int ti = q * tws;
+#pragma unroll
+        for (int m = 1; m < R; m++) p[m * Q * pitch] = ti ? cmul(a[m], tw[m * ti]) : a[m];
+    }
+    __syncthreads();
+}
+
+// in-place forward DIF of B lines held at sm[n * pitch + b]; all threads of the CTA call (it ends with a barrier)
+template <typename T, typename C, int B>
+__device__ __forceinline__ void mr_fft_tile(C *sm, const C *tw, const MixedPlan &plan, int twmul) {
+    int Ns = plan.n;
+    for (int s = 0; s < plan.nstage; s++) {
+        const int R = mr_radix(plan, s);
+        switch (R) {
+            case 8: mr_stage<T, C, B, 8>(sm, tw, plan.n, Ns, twmul); break;
+            case 4: mr_stage<T, C, B, 4>(sm, tw, plan.n, Ns, twmul); break;
+            case 2: mr_stage<T, C, B, 2>(sm, tw, plan.n, Ns, twmul); break;
+            case 3: mr_stage<T, C, B, 3>(sm, tw, plan.n, Ns, twmul); break;
+            case 5: mr_stage<T, C, B, 5>(sm, tw, plan.n, Ns, twmul); break;
+            default: mr_stage<T, C, B, 7>(sm, tw, plan.n, Ns, twmul); break;
+        }
+        Ns /= R;
+    }
+}
+
+// perm[k] = position of frequency k after mr_fft_tile (mixed-radix digit reversal).  No barrier.
+__device__ __forceinline__ void mr_build_perm(unsigned short *perm, const MixedPlan &plan) {
+    for (int k = threadIdx.x; k < plan.n; k += blockDim.x) {
+        int rem = k, base = plan.n, pos = 0;
+        for (int s = 0; s < plan.nstage; s++) {
+            const int R = mr_radix(plan, s);
+            const int d = rem % R;
+            rem /= R;
+            base /= R;
+            pos += d * base;
+        }
+        perm[k] = (unsigned short)pos;
+    }
+}
+
+// strided tile -> shared [N][pitch] with cp.async; columns beyond the valid width are zero-filled with plain stores
+template <typename C, int B>
+__device__ __forceinline__ void mr_prefetch_tile(C *sm, const C *base, int N, int64_t line_stride, int bvalid) {
+    constexpr int pitch = MrPitch<B>::v;
+    for (int w = threadIdx.x; w < N * B; w += blockDim.x) {
+        const int b = w % B, n = w / B;
+        if (b < bvalid) cp_async_elem(&sm[n * pitch + b], base + (int64_t)n * line_stride + b);
+        else sm[n * pitch + b] = C{0, 0};
+    }
+}
+
+// strided line pass, element(outer, n, inner) = data[outer * outer_stride + n * line_stride + inner].  dst == src: in
+// place (a CTA reads its whole tile before it stores any of it).
+// shared: buf[2][N][pitch] | W_N^i [N] | perm ushort[N]
+template <typename T, int B>
+__global__ void __launch_bounds__(512)
+k_fft_lines_mixed(const typename C2<T>::type *src, typename C2<T>::type *dst, const typename C2<T>::type *__restrict__ tw_g,
+                  MixedPlan plan, int64_t line_stride, int64_t n_inner, int64_t tiles_inner, int64_t n_tiles,
+                  int64_t outer_stride, int inverse, T scale) {
+    typedef typename C2<T>::type C;
+    constexpr int pitch = MrPitch<B>::v;
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const int N = plan.n;
+    C *buf0 = reinterpret_cast<C *>(smem_raw);
+    C *buf1 = buf0 + (size_t)N * pitch;
+    C *tw = buf1 + (size_t)N * pitch;
+    unsigned short *perm = reinterpret_cast<unsigned short *>(tw + N);
+    for (int i = threadIdx.x; i < N; i += blockDim.x) tw[i] = tw_g[i];
+    mr_build_perm(perm, plan);
+    int64_t tile = blockIdx.x;
+    if (tile < n_tiles) {
+        const int64_t outer = tile / tiles_inner;
+        const int64_t inner0 = (tile - outer * tiles_inner) * B;
+        const int bvalid = (int)((n_inner - inner0) < B ? (n_inner - inner0) : B);
+        mr_prefetch_tile<C, B>(buf0, src + outer * outer_stride + inner0, N, line_stride, bvalid);
+    }
+    cp_async_commit();
+    int cur = 0;
+    for (; tile < n_tiles; tile += gridDim.x, cur ^= 1) {
+        C *sm = cur ? buf1 : buf0;
+        const int64_t outer = tile / tiles_inner;
+        const int64_t inner0 = (tile - outer * tiles_inner) * B;
+        C *obase = dst + outer * outer_stride + inner0;
+        const int bvalid = (int)((n_inner - inner0) < B ? (n_inner - inner0) : B);
+        const int64_t nxt = tile + gridDim.x;
+        if (nxt < n_tiles) {
+            const int64_t o2 = nxt / tiles_inner;
+            const int64_t i2 = (nxt - o2 * tiles_inner) * B;
+            const int bv2 = (int)((n_inner - i2) < B ? (n_inner - i2) : B);
+            mr_prefetch_tile<C, B>(cur ? buf0 : buf1, src + o2 * outer_stride + i2, N, line_stride, bv2);
+        }
+        cp_async_commit();
+        cp_async_wait<1>();          // this tile's copies have landed (the prefetch may still be in flight)
+        __syncthreads();             // (the first time through also publishes tw and perm)
+        mr_fft_tile<T, C, B>(sm, tw, plan, 1);
+        for (int w = threadIdx.x; w < N * B; w += blockDim.x) {
+            const int b = w % B, k = w / B;
+            if (b < bvalid) {
+                const int kk = (inverse && k) ? N - k : k;
+                const C v = sm[perm[kk] * pitch + b];
+                obase[(int64_t)k * line_stride + b] = C{v.x * scale, v.y * scale};
+            }
+        }
+        __syncthreads();             // everyone is done with `sm` before the next prefetch overwrites it
+    }
+    cp_async_wait<0>();
+}
+
+// z pass: real rows [rows][Nz] <-> complex rows [rows][Nz/2+1].  A tile holds B complex lines of plan.n points: one
+// row each (even Nz, n = Nz/2, packed pairs) or two rows each (odd Nz, n = Nz, row 2b in re, row 2b+1 in im).
+// shared: tile [n][pitch] | W_Nz^i [Nz] | perm ushort[n].  Forward scaled by `scale`, inverse unnormalised times `scale`.
+template <typename T, int B>
+__global__ void __launch_bounds__(256)
+k_fft_z_mixed(const void *in, void *out, const typename C2<T>::type *__restrict__ tw_g, MixedPlan plan, int Nz,
+              int64_t rows, int inverse, T scale) {
+    typedef typename C2<T>::type C;
+    constexpr int pitch = MrPitch<B>::v;
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const int L = plan.n;
+    const bool odd = Nz & 1;
+    const int Nzc = Nz / 2 + 1;
+    const int rpl = odd ? 2 : 1;                   // real rows per complex line
+    C *sm = reinterpret_cast<C *>(smem_raw);
+    C *tw = sm + (size_t)L * pitch;
+    unsigned short *perm = reinterpret_cast<unsigned short *>(tw + Nz);
+    for (int i = threadIdx.x; i < Nz; i += blockDim.x) tw[i] = tw_g[i];
+    mr_build_perm(perm, plan);
+    __syncthreads();
+    const int64_t per_tile = (int64_t)B * rpl;
+    const int64_t n_tiles = (rows + per_tile - 1) / per_tile;
+    const T h = (T)0.5 * scale;
+    for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        const int64_t row0 = tile * per_tile;
+        const int nrows = (int)((rows - row0) < per_tile ? (rows - row0) : per_tile);
+        // ---- load (lanes along the contiguous rows)
+        if (!inverse && !odd) {
+            const C *src = reinterpret_cast<const C *>(static_cast<const T *>(in) + row0 * Nz);
+            for (int w = threadIdx.x; w < L * B; w += blockDim.x) {
+                const int b = w / L, n = w - b * L;
+                sm[n * pitch + b] = b < nrows ? src[(int64_t)b * L + n] : C{0, 0};
+            }
+        } else if (!inverse) {
+            const T *src = static_cast<const T *>(in) + row0 * Nz;
+            for (int w = threadIdx.x; w < L * B; w += blockDim.x) {
+                const int b = w / L, n = w - b * L;
+                const T xa = 2 * b < nrows ? src[(int64_t)(2 * b) * Nz + n] : (T)0;
+                const T xb = 2 * b + 1 < nrows ? src[(int64_t)(2 * b + 1) * Nz + n] : (T)0;
+                sm[n * pitch + b] = C{xa, xb};
+            }
+        } else if (!odd) {
+            // Z[k] = E + i O,  E = X[k] + conj X[M-k],  O = conj(W_Nz^k) (X[k] - conj X[M-k]),  k < M  (the factor 1/2 of
+            // the split and the 2 of the unnormalised inverse cancel)
+            const C *src = static_cast<const C *>(in) + row0 * Nzc;
+            for (int w = threadIdx.x; w < L * B; w += blockDim.x) {
+                const int b = w / L, k = w - b * L;
+                C z = C{0, 0};
+                if (b < nrows) {
+                    const C xk = src[(int64_t)b * Nzc + k];
+                    const C xm = cconj(src[(int64_t)b * Nzc + (L - k)]);
+                    const C e = cadd(xk, xm), d = csub(xk, xm);
+                    const C o = cmul(cconj(tw[k]), d);
+                    z = C{e.x - o.y, e.y + o.x};
+                }
+                sm[k * pitch + b] = z;
+            }
+        } else {
+            // both Hermitian rows rebuilt in the tile: Z[k] = X_a[k] + i X_b[k], Z[Nz-k] = conj X_a[k] + i conj X_b[k]
+            const C *src = static_cast<const C *>(in) + row0 * Nzc;
+            for (int w = threadIdx.x; w < Nzc * B; w += blockDim.x) {
+                const int b = w / Nzc, k = w - b * Nzc;
+                C A = 2 * b < nrows ? src[(int64_t)(2 * b) * Nzc + k] : C{0, 0};
+                C Bv = 2 * b + 1 < nrows ? src[(int64_t)(2 * b + 1) * Nzc + k] : C{0, 0};
+                if (k == 0) { A.y = 0; Bv.y = 0; }          // the k = 0 mode of a real row is real
+                sm[k * pitch + b] = C{A.x - Bv.y, A.y + Bv.x};
+                if (k) sm[(L - k) * pitch + b] = C{A.x + Bv.y, Bv.x - A.y};
+            }
+        }
+        __syncthreads();
+        mr_fft_tile<T, C, B>(sm, tw, plan, odd ? 1 : 2);
+        // ---- store
+        if (!inverse && !odd) {
+            // X[k] = 1/2 [ (Z[k] + conj Z[M-k]) - i W_Nz^k (Z[k] - conj Z[M-k]) ],  k = 0 .. M  (Z[M] := Z[0])
+            C *dst = static_cast<C *>(out) + row0 * Nzc;
+            for (int w = threadIdx.x; w < Nzc * B; w += blockDim.x) {
+                const int b = w / Nzc, k = w - b * Nzc;
+                if (b < nrows) {
+                    const C zk = sm[perm[k == L ? 0 : k] * pitch + b];
+                    const C zm = cconj(sm[perm[k == 0 ? 0 : L - k] * pitch + b]);
+                    const C e = cadd(zk, zm), o = csub(zk, zm);
+                    const C wo = cmul(tw[k], o);
+                    dst[(int64_t)b * Nzc + k] = C{(e.x + wo.y) * h, (e.y - wo.x) * h};
+                }
+            }
+        } else if (!inverse) {
+            // X_a[k] = (Z[k] + conj Z[-k]) / 2,  X_b[k] = -i (Z[k] - conj Z[-k]) / 2
+            C *dst = static_cast<C *>(out) + row0 * Nzc;
+            for (int w = threadIdx.x; w < Nzc * B; w += blockDim.x) {
+                const int b = w / Nzc, k = w - b * Nzc;
+                if (2 * b < nrows) {
+                    const C zk = sm[perm[k] * pitch + b];
+                    const C zm = cconj(sm[perm[k ? L - k : 0] * pitch + b]);
+                    const C e = cadd(zk, zm), d = csub(zk, zm);
+                    dst[(int64_t)(2 * b) * Nzc + k] = C{e.x * h, e.y * h};
+                    if (2 * b + 1 < nrows) dst[(int64_t)(2 * b + 1) * Nzc + k] = C{d.y * h, -d.x * h};
+                }
+            }
+        } else if (!odd) {
+            // x[2n] + i x[2n+1] = sum_k Z[k] e^{+2 pi i k n / M} = DFT(Z)[(M - n) mod M]
+            C *dst = reinterpret_cast<C *>(static_cast<T *>(out) + row0 * Nz);
+            for (int w = threadIdx.x; w < L * B; w += blockDim.x) {
+                const int b = w / L, n = w - b * L;
+                if (b < nrows) {
+                    const C v = sm[perm[n ? L - n : 0] * pitch + b];
+                    dst[(int64_t)b * L + n] = C{v.x * scale, v.y * scale};
+                }
+            }
+        } else {
+            T *dst = static_cast<T *>(out) + row0 * Nz;
+            for (int w = threadIdx.x; w < L * B; w += blockDim.x) {
+                const int b = w / L, n = w - b * L;
+                if (2 * b < nrows) {
+                    const C v = sm[perm[n ? L - n : 0] * pitch + b];
+                    dst[(int64_t)(2 * b) * Nz + n] = v.x * scale;
+                    if (2 * b + 1 < nrows) dst[(int64_t)(2 * b + 1) * Nz + n] = v.y * scale;
+                }
+            }
+        }
+        __syncthreads();
+    }
+}
+
+// ---- host side
+static bool is_7smooth(int64_t n) {
+    if (n < 1) return false;
+    for (int p : {2, 3, 5, 7})
+        while (n % p == 0) n /= p;
+    return n == 1;
+}
+
+static MixedPlan mr_plan(int n) {
+    MixedPlan p;
+    p.n = n;
+    p.nstage = 0;
+    p.radices = 0;
+    auto push = [&](int r) { p.radices |= (unsigned long long)r << (4 * p.nstage); p.nstage++; };
+    int m = n, c2 = 0;
+    while (m % 2 == 0) { m /= 2; c2++; }
+    for (; c2 >= 3; c2 -= 3) push(8);
+    if (c2 == 2) push(4);
+    else if (c2 == 1) push(2);
+    for (int r : {7, 5, 3})
+        while (m % r == 0) { m /= r; push(r); }
+    return p;
+}
+
+// complex line length n (2 .. 4096, 7-smooth)
+static int check_line_mixed(const char *who, int64_t n) {
+    NBK_CHECK_ARG(n >= 2 && n <= NBK_MR_MAX_LINE && is_7smooth(n),
+                  "%s: line length %lld unsupported: the mixed-radix FFT takes lengths 2 .. 4096 whose prime factors are "
+                  "2, 3, 5 and 7", who, (long long)n);
+    return NBK_OK;
+}
+
+static int check_z_mixed(const char *who, int64_t Nz) {
+    NBK_CHECK_ARG(Nz >= 2 && is_7smooth(Nz) && ((Nz % 2 == 0 && Nz <= 2 * NBK_MR_MAX_LINE) || (Nz % 2 && Nz < NBK_MR_MAX_LINE)),
+                  "%s: Nz = %lld unsupported: the mixed-radix z pass takes 7-smooth lengths (prime factors 2, 3, 5, 7), "
+                  "even up to 8192 or odd up to 4095", who, (long long)Nz);
+    return NBK_OK;
+}
+
+static int check_dims_mixed(const char *who, int dtype, const int64_t *nmesh) {
+    NBK_CHECK_ARG(dtype == NBK_F4 || dtype == NBK_F8, "%s: bad dtype %d", who, dtype);
+    const int64_t Nx = nmesh[0], Ny = nmesh[1], Nz = nmesh[2];
+    const bool zok = Nz >= 2 && is_7smooth(Nz) && ((Nz % 2 == 0 && Nz <= 2 * NBK_MR_MAX_LINE) || (Nz % 2 && Nz < NBK_MR_MAX_LINE));
+    NBK_CHECK_ARG(Nx >= 2 && Ny >= 2 && Nx <= NBK_MR_MAX_LINE && Ny <= NBK_MR_MAX_LINE && is_7smooth(Nx) && is_7smooth(Ny) && zok,
+                  "%s: Nmesh (%lld,%lld,%lld) unsupported: each side must be a product of 2, 3, 5 and 7 (Nx, Ny 2 .. 4096; "
+                  "Nz 2 .. 8192 if even, up to 4095 if odd)", who, (long long)Nx, (long long)Ny, (long long)Nz);
+    return NBK_OK;
+}
+
+template <typename T>
+static int launch_lines_mixed(const void *src, void *dst, int N, int64_t line_stride, int64_t n_inner, int64_t n_outer,
+                              int64_t outer_stride, int inverse, double scale, cudaStream_t s) {
+    typedef typename C2<T>::type C;
+    const int dtype = sizeof(T) == 4 ? NBK_F4 : NBK_F8;
+    void *tw;
+    int rc = get_twiddle(N, dtype, s, &tw);
+    if (rc) return rc;
+    // two tile buffers + twiddles + digit-reversal table; 128-byte runs while that fits, narrower for long lines
+    auto smem_for = [&](int B) { return (size_t)N * (2 * (B > 1 ? B + 1 : 1) + 1) * sizeof(C) + (size_t)N * 2 + 16; };
+    int B = 128 / (int)sizeof(C);
+    while (B > 1 && (smem_for(B) > 220 * 1024 || B / 2 >= n_inner)) B >>= 1;
+    const size_t smem = smem_for(B);
+    NBK_CHECK_ARG(smem <= 227 * 1024, "fft_lines_mixed: N=%d does not fit in shared memory", N);
+    const int64_t tiles_inner = (n_inner + B - 1) / B;
+    const int64_t n_tiles = tiles_inner * n_outer;
+    int per_sm = (int)((227 * 1024) / (smem + 1024));
+    if (per_sm < 1) per_sm = 1;
+    if (per_sm > 8) per_sm = 8;
+    const int64_t g = n_tiles < (int64_t)NBK_SM_COUNT * per_sm ? n_tiles : (int64_t)NBK_SM_COUNT * per_sm;
+    const int nthreads = (per_sm == 1 && (int64_t)N * B >= 4096) ? 512 : 256;
+    const MixedPlan plan = mr_plan(N);
+#define LAUNCH_LM(BB)                                                                                              \
+    case BB:                                                                                                       \
+        NBK_CUDA(cudaFuncSetAttribute(k_fft_lines_mixed<T, BB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+        k_fft_lines_mixed<T, BB><<<(int)g, nthreads, smem, s>>>((const C *)src, (C *)dst, (const C *)tw, plan, line_stride, \
+                                                                 n_inner, tiles_inner, n_tiles, outer_stride, inverse, (T)scale); \
+        break;
+    switch (B) {
+        LAUNCH_LM(1) LAUNCH_LM(2) LAUNCH_LM(4) LAUNCH_LM(8) LAUNCH_LM(16)
+        default: nbk_set_error("fft_lines_mixed: internal tile width %d", B); return NBK_ERR_ARG;
+    }
+#undef LAUNCH_LM
+    NBK_LAUNCHED();
+    return NBK_OK;
+}
+
+template <typename T>
+static int launch_z_mixed(const void *in, void *out, int64_t rows, int Nz, int inverse, double scale, cudaStream_t s) {
+    typedef typename C2<T>::type C;
+    const int dtype = sizeof(T) == 4 ? NBK_F4 : NBK_F8;
+    void *tw;
+    int rc = get_twiddle(Nz, dtype, s, &tw);
+    if (rc) return rc;
+    const bool odd = Nz & 1;
+    const int L = odd ? Nz : Nz / 2;
+    const int64_t lines = odd ? (rows + 1) / 2 : rows;
+    // B rows per tile: as many as leave two CTAs per SM (one CTA's loads overlap the other's butterflies); long rows
+    // take the whole SM
+    auto smem_for = [&](int B) { return ((size_t)L * (B > 1 ? B + 1 : 1) + Nz) * sizeof(C) + (size_t)L * 2 + 16; };
+    int B = 16;
+    while (B > 1 && (smem_for(B) > 110 * 1024 || B / 2 >= lines)) B >>= 1;
+    const size_t smem = smem_for(B);
+    NBK_CHECK_ARG(smem <= 227 * 1024, "fft_z_mixed: Nz=%d does not fit in shared memory", Nz);
+    const int64_t n_tiles = (lines + B - 1) / B;
+    int per_sm = (int)((227 * 1024) / (smem + 1024));
+    if (per_sm < 1) per_sm = 1;
+    if (per_sm > 8) per_sm = 8;
+    const int64_t g = n_tiles < (int64_t)NBK_SM_COUNT * per_sm ? n_tiles : (int64_t)NBK_SM_COUNT * per_sm;
+    const MixedPlan plan = mr_plan(L);
+#define LAUNCH_ZM(BB)                                                                                              \
+    case BB:                                                                                                       \
+        NBK_CUDA(cudaFuncSetAttribute(k_fft_z_mixed<T, BB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+        k_fft_z_mixed<T, BB><<<(int)g, 256, smem, s>>>(in, out, (const C *)tw, plan, Nz, rows, inverse, (T)scale); \
+        break;
+    switch (B) {
+        LAUNCH_ZM(1) LAUNCH_ZM(2) LAUNCH_ZM(4) LAUNCH_ZM(8) LAUNCH_ZM(16)
+        default: nbk_set_error("fft_z_mixed: internal tile width %d", B); return NBK_ERR_ARG;
+    }
+#undef LAUNCH_ZM
+    NBK_LAUNCHED();
+    return NBK_OK;
+}
+
+extern "C" int nbk_fft_lines_mixed(const void *src, void *dst, int dtype, int64_t n_line, int64_t line_stride, int64_t n_inner,
+                                   int64_t n_outer, int64_t outer_stride, int inverse, double scale, void *stream) {
+    NBK_CHECK_ARG(dtype == NBK_F4 || dtype == NBK_F8, "fft_lines_mixed: bad dtype %d", dtype);
+    int rc = check_line_mixed("fft_lines_mixed", n_line);
+    if (rc) return rc;
+    if (n_inner <= 0 || n_outer <= 0) return NBK_OK;
+    cudaStream_t s = (cudaStream_t)stream;
+    if (dtype == NBK_F4)
+        return launch_lines_mixed<float>(src, dst, (int)n_line, line_stride, n_inner, n_outer, outer_stride, inverse, scale, s);
+    return launch_lines_mixed<double>(src, dst, (int)n_line, line_stride, n_inner, n_outer, outer_stride, inverse, scale, s);
+}
+
+extern "C" int nbk_fft_z_mixed(const void *in, void *out, int dtype, int64_t rows, int64_t Nz, int inverse, double scale,
+                               void *stream) {
+    NBK_CHECK_ARG(dtype == NBK_F4 || dtype == NBK_F8, "fft_z_mixed: bad dtype %d", dtype);
+    int rc = check_z_mixed("fft_z_mixed", Nz);
+    if (rc) return rc;
+    if (rows <= 0) return NBK_OK;
+    cudaStream_t s = (cudaStream_t)stream;
+    return (dtype == NBK_F4) ? launch_z_mixed<float>(in, out, rows, (int)Nz, inverse, scale, s)
+                             : launch_z_mixed<double>(in, out, rows, (int)Nz, inverse, scale, s);
+}
+
+extern "C" int nbk_r2c_mixed(const void *real, void *cplx, int dtype, const int64_t *nmesh, double extra_scale, void *stream) {
+    int rc = check_dims_mixed("r2c_mixed", dtype, nmesh);
+    if (rc) return rc;
+    const int64_t Nx = nmesh[0], Ny = nmesh[1], Nz = nmesh[2], Nzc = Nz / 2 + 1;
+    rc = nbk_fft_z_mixed(real, cplx, dtype, Nx * Ny, Nz, 0, 1.0, stream);
+    if (rc) return rc;
+    rc = nbk_fft_lines_mixed(cplx, cplx, dtype, Ny, Nzc, Nzc, Nx, Ny * Nzc, 0, 1.0, stream);
+    if (rc) return rc;
+    const double scale = extra_scale / ((double)Nx * (double)Ny * (double)Nz);
+    return nbk_fft_lines_mixed(cplx, cplx, dtype, Nx, Ny * Nzc, Ny * Nzc, 1, 0, 0, scale, stream);
+}
+
+// c2r destroys its complex input unless `work` (same size as cplx) is given
+extern "C" int nbk_c2r_mixed(const void *cplx, void *real, int dtype, const int64_t *nmesh, void *work, void *stream) {
+    int rc = check_dims_mixed("c2r_mixed", dtype, nmesh);
+    if (rc) return rc;
+    const int64_t Nx = nmesh[0], Ny = nmesh[1], Nz = nmesh[2], Nzc = Nz / 2 + 1;
+    void *c = const_cast<void *>(cplx);
+    if (work && work != cplx) {
+        const size_t bytes = (size_t)Nx * Ny * Nzc * (dtype == NBK_F4 ? 8 : 16);
+        NBK_CUDA(cudaMemcpyAsync(work, cplx, bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+        c = work;
+    }
+    rc = nbk_fft_lines_mixed(c, c, dtype, Nx, Ny * Nzc, Ny * Nzc, 1, 0, 1, 1.0, stream);
+    if (rc) return rc;
+    rc = nbk_fft_lines_mixed(c, c, dtype, Ny, Nzc, Nzc, Nx, Ny * Nzc, 1, 1.0, stream);
+    if (rc) return rc;
+    return nbk_fft_z_mixed(c, real, dtype, Nx * Ny, Nz, 1, 1.0, stream);
 }

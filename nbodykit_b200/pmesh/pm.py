@@ -241,6 +241,9 @@ class ParticleMesh(object):
         self.y_start = self.comm.rank * self.y_n
         self.Nzc = Nz if self.cplx else Nz // 2 + 1      # stored length of the last axis of a ComplexField
         self.transposed = P > 1
+        # every side a power of two: the radix-8 kernels (and, with P > 1, the NVLink peer transpose); otherwise the
+        # mixed-radix transform, whose entry points check the sizes it takes (products of 2, 3, 5 and 7)
+        self.pow2 = all(n > 0 and n & (n - 1) == 0 for n in (Nx, Ny, Nz))
         self._nmesh_c = iarr(self.Nmesh)
         self._box_c = darr(self.BoxSize)
         self._coords = {}
@@ -877,6 +880,8 @@ class RealField(Field):
         pm = self.pm
         if out is None or out is Ellipsis:
             out = ComplexField(pm)
+        if not pm.pow2:
+            return self._r2c_mixed(out, scale)
         code = _CODE[pm.typestr]
         P = pm.comm.size
         Nx, Ny, Nz = [int(v) for v in pm.Nmesh]
@@ -964,6 +969,44 @@ class RealField(Field):
         out.attrs = dict(self.attrs)
         return out
 
+    def _r2c_mixed(self, out, scale):
+        """r2c for sides that are not all powers of two (mixed-radix kernels).  P > 1: z pass, y lines, pack, NCCL
+        all-to-all, unpack, x lines with the normalisation"""
+        pm = self.pm
+        L = lib()
+        code = _CODE[pm.typestr]
+        P = pm.comm.size
+        Nx, Ny, Nz = [int(v) for v in pm.Nmesh]
+        if pm.cplx:
+            half = torch.empty((Nx, Ny, Nz // 2 + 1), dtype=out.value.dtype, device=out.value.device)
+            with stage("r2c"):
+                check(L.nbk_r2c_mixed(_ptr(self.value), _ptr(half), code, pm._nmesh_c, float(scale), _stream()), "nbk_r2c_mixed")
+                check(L.nbk_hermitian_expand(_ptr(half), _ptr(out.value), code, pm._nmesh_c, _stream()), "nbk_hermitian_expand")
+        elif P == 1:
+            with stage("r2c"):
+                check(L.nbk_r2c_mixed(_ptr(self.value), _ptr(out.value), code, pm._nmesh_c, float(scale), _stream()), "nbk_r2c_mixed")
+        else:
+            Nzc = pm.Nzc
+            work = torch.empty((pm.x_n, Ny, Nzc), dtype=out.value.dtype, device=out.value.device)
+            send = torch.empty_like(work)
+            with stage("fft_zy"):
+                check(L.nbk_fft_z_mixed(_ptr(self.value), _ptr(work), code, pm.x_n * Ny, Nz, 0, 1.0, _stream()), "fft_z_mixed")
+                check(L.nbk_fft_lines_mixed(_ptr(work), _ptr(work), code, Ny, Nzc, Nzc, pm.x_n, Ny * Nzc, 0, 1.0, _stream()),
+                      "fft_lines_mixed(y)")
+            with stage("fft_pack"):
+                check(L.nbk_transpose_pack(_ptr(work), _ptr(send), code, pm.x_n, Ny, Nzc, P, _stream()), "transpose_pack")
+            recv = torch.view_as_real(work).view(-1)
+            with stage("fft_alltoall"):
+                pm.comm.all_to_all_single(recv, torch.view_as_real(send).view(-1))
+            with stage("fft_unpack"):
+                check(L.nbk_transpose_unpack(_ptr(recv), _ptr(out.value), code, pm.y_n, Nx, Nzc, P, _stream()), "transpose_unpack")
+            scale = float(scale) / (float(Nx) * Ny * Nz)
+            with stage("fft_x"):
+                check(L.nbk_fft_lines_mixed(_ptr(out.value), _ptr(out.value), code, Nx, Nzc, Nzc, pm.y_n, Nx * Nzc, 0, scale,
+                                            _stream()), "fft_lines_mixed(x)")
+        out.attrs = dict(self.attrs)
+        return out
+
 
 class BaseComplexField(Field):
     pass
@@ -998,6 +1041,8 @@ class ComplexField(BaseComplexField):
         pm = self.pm
         if out is None or out is Ellipsis:
             out = RealField(pm)
+        if not pm.pow2:
+            return self._c2r_mixed(out)
         code = _CODE[pm.typestr]
         P = pm.comm.size
         Nx, Ny, Nz = [int(v) for v in pm.Nmesh]
@@ -1049,6 +1094,42 @@ class ComplexField(BaseComplexField):
             slab = torch.view_as_real(send).view(-1)
             check(lib().nbk_transpose_unpack_back(_ptr(recv), _ptr(slab), code, pm.x_n, Ny, Nzc, P, _stream()), "unpack_back")
             check(lib().nbk_fft_zy_backward(_ptr(slab), _ptr(out.value), code, pm.x_n, Ny, Nz, _stream()), "fft_zy_backward")
+        out.attrs = dict(self.attrs)
+        return out
+
+    def _c2r_mixed(self, out):
+        """c2r for sides that are not all powers of two (mixed-radix kernels), the mirror of RealField._r2c_mixed.
+        The complex buffer is preserved."""
+        pm = self.pm
+        L = lib()
+        code = _CODE[pm.typestr]
+        P = pm.comm.size
+        Nx, Ny, Nz = [int(v) for v in pm.Nmesh]
+        if pm.cplx:
+            half = torch.empty((Nx, Ny, Nz // 2 + 1), dtype=self.value.dtype, device=self.value.device)
+            with stage("c2r"):
+                check(L.nbk_hermitian_compress(_ptr(self.value), _ptr(half), code, Nx * Ny, Nz, _stream()), "nbk_hermitian_compress")
+                check(L.nbk_c2r_mixed(_ptr(half), _ptr(out.value), code, pm._nmesh_c, None, _stream()), "nbk_c2r_mixed")
+        elif P == 1:
+            work = torch.empty_like(self.value)
+            with stage("c2r"):
+                check(L.nbk_c2r_mixed(_ptr(self.value), _ptr(out.value), code, pm._nmesh_c, _ptr(work), _stream()), "nbk_c2r_mixed")
+        else:
+            Nzc = pm.Nzc
+            work = self.value.clone()
+            with stage("ifft_x"):
+                check(L.nbk_fft_lines_mixed(_ptr(work), _ptr(work), code, Nx, Nzc, Nzc, pm.y_n, Nx * Nzc, 1, 1.0, _stream()),
+                      "fft_lines_mixed(x)")
+            send = torch.empty_like(work)
+            check(L.nbk_transpose_pack_back(_ptr(work), _ptr(send), code, pm.y_n, Nx, Nzc, P, _stream()), "pack_back")
+            recv = torch.view_as_real(work).view(-1)
+            pm.comm.all_to_all_single(recv, torch.view_as_real(send).view(-1))
+            slab = torch.view_as_real(send).view(-1)
+            check(L.nbk_transpose_unpack_back(_ptr(recv), _ptr(slab), code, pm.x_n, Ny, Nzc, P, _stream()), "unpack_back")
+            with stage("ifft_zy"):
+                check(L.nbk_fft_lines_mixed(_ptr(slab), _ptr(slab), code, Ny, Nzc, Nzc, pm.x_n, Ny * Nzc, 1, 1.0, _stream()),
+                      "fft_lines_mixed(y)")
+                check(L.nbk_fft_z_mixed(_ptr(slab), _ptr(out.value), code, pm.x_n * Ny, Nz, 1, 1.0, _stream()), "fft_z_mixed")
         out.attrs = dict(self.attrs)
         return out
 

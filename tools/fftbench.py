@@ -1,25 +1,115 @@
-"""r2c / c2r timing only (scratch)."""
-import sys, os
-import numpy as np, torch
+"""Whole-mesh r2c / c2r timing on one GPU, one JSON line per case.
+
+    python tools/fftbench.py                          # the default case list below
+    python tools/fftbench.py 96:f8 768:f4:r2c         # side:dtype[:r2c] -- ':r2c' skips the c2r (it needs a third field)
+
+Every case is timed with CUDA events after warm-up (median of --reps calls).  Effective bandwidth counts 6x the real
+field's bytes per transform (three passes, each one read and one write of a field of about that size) and is compared
+with the 3.35 TB/s HBM3 data-sheet figure of the H100 SXM.  For sides that are not powers of two the three passes of
+the mixed-radix r2c (z, y, x) are also timed one by one.  The card's name and power limit are printed with the numbers.
+"""
+import argparse
+import ctypes
+import json
+import os
+import subprocess
+import sys
+
+import torch
+
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from nbodykit_b200.pmesh.pm import ParticleMesh, RealField, ComplexField
-from nbodykit_b200.comm import SelfComm
-N = int(sys.argv[1]) if len(sys.argv) > 1 else 512
-dt = sys.argv[2] if len(sys.argv) > 2 else "f8"
-pm = ParticleMesh(BoxSize=1.0, Nmesh=N, dtype=dt, comm=SelfComm())
-r = RealField(pm); r.value.normal_()
-c = ComplexField(pm)
-def t(fn, n=5):
-    for _ in range(2): fn()
+from nbodykit_b200 import _lib  # noqa: E402
+from nbodykit_b200.comm import SelfComm  # noqa: E402
+from nbodykit_b200.pmesh.pm import ComplexField, ParticleMesh, RealField  # noqa: E402
+
+DEFAULT = ["512:f8", "768:f8", "1000:f8", "1024:f8", "1536:f4", "1536:f8:r2c"]
+HBM_PEAK = 3.35e12
+
+
+def _card():
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
+        power, clock = [s.strip() for s in q[torch.cuda.current_device()].split(",")]
+    except Exception:       # noqa: BLE001  (no nvidia-smi: the numbers still stand, the power limit is unknown)
+        power, clock = "unknown", "unknown"
+    return dict(gpu=torch.cuda.get_device_name(), power_limit=power, max_sm_clock=clock)
+
+
+def _time(fn, warmup, reps):
+    for _ in range(warmup):
+        fn()
     torch.cuda.synchronize()
-    best = 1e9
-    for _ in range(n):
+    ts = []
+    for _ in range(reps):
         a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record(); fn(); b.record(); torch.cuda.synchronize()
-        best = min(best, a.elapsed_time(b))
-    return best
-fb = r.value.numel() * r.value.element_size()
-ms = t(lambda: r.r2c(out=c))
-print("r2c %d^3 %s: %.3f ms (6x field bytes moved / t = %.0f GB/s; 4x = %.0f GB/s)" % (N, dt, ms, 6 * fb / ms / 1e6, 4 * fb / ms / 1e6))
-ms = t(lambda: c.c2r(out=r))
-print("c2r %d^3 %s: %.3f ms" % (N, dt, ms))
+        a.record()
+        fn()
+        b.record()
+        torch.cuda.synchronize()
+        ts.append(a.elapsed_time(b))
+    ts.sort()
+    return ts[len(ts) // 2]
+
+
+def _passes(pm, r, c, warmup, reps):
+    """ms of the z pass, the y lines and the x lines of the mixed-radix r2c"""
+    L = _lib.lib()
+    code = 4 if pm.typestr == "f4" else 8
+    Nx, Ny, Nz = [int(v) for v in pm.Nmesh]
+    Nzc = Nz // 2 + 1
+    rp, cp = ctypes.c_void_p(r.value.data_ptr()), ctypes.c_void_p(c.value.data_ptr())
+    out = {}
+    out["z"] = _time(lambda: _lib.check(L.nbk_fft_z_mixed(rp, cp, code, Nx * Ny, Nz, 0, 1.0, None)), warmup, reps)
+    out["y"] = _time(lambda: _lib.check(L.nbk_fft_lines_mixed(cp, cp, code, Ny, Nzc, Nzc, Nx, Ny * Nzc, 0, 1.0, None)),
+                     warmup, reps)
+    out["x"] = _time(lambda: _lib.check(L.nbk_fft_lines_mixed(cp, cp, code, Nx, Ny * Nzc, Ny * Nzc, 1, 0, 0, 1.0, None)),
+                     warmup, reps)
+    return {k: round(v, 3) for k, v in out.items()}
+
+
+def run_case(spec, warmup, reps, card):
+    parts = spec.split(":")
+    n, dtype = int(parts[0]), parts[1]
+    with_c2r = not (len(parts) > 2 and parts[2] == "r2c")
+    pm = ParticleMesh(BoxSize=1.0, Nmesh=n, dtype=dtype, comm=SelfComm())
+    r = RealField(pm)
+    r.value.normal_()
+    c = ComplexField(pm)
+    field_bytes = r.value.numel() * r.value.element_size()
+    res = dict(case="r2c+c2r" if with_c2r else "r2c", Nmesh=n, dtype=dtype, path="power-of-two" if pm.pow2 else "mixed-radix")
+    ms = _time(lambda: r.r2c(out=c), warmup, reps)
+    res["r2c_ms"] = round(ms, 3)
+    res["r2c_ns_per_cell"] = round(ms * 1e6 / n ** 3, 4)
+    res["r2c_GBps"] = round(6 * field_bytes / (ms * 1e-3) / 1e9, 1)
+    res["r2c_frac_hbm_peak"] = round(6 * field_bytes / (ms * 1e-3) / HBM_PEAK, 3)
+    if not pm.pow2:
+        res["r2c_passes_ms"] = _passes(pm, r, c, warmup, reps)
+    if with_c2r:
+        ms = _time(lambda: c.c2r(out=r), warmup, reps)
+        res["c2r_ms"] = round(ms, 3)
+        res["c2r_GBps"] = round(6 * field_bytes / (ms * 1e-3) / 1e9, 1)
+        res["c2r_frac_hbm_peak"] = round(6 * field_bytes / (ms * 1e-3) / HBM_PEAK, 3)
+    res.update(card)
+    print(json.dumps(res), flush=True)
+    del r, c
+    torch.cuda.empty_cache()
+    return res
+
+
+def main():
+    ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
+    ap.add_argument("cases", nargs="*", default=DEFAULT, help="side:dtype[:r2c] (default: %s)" % " ".join(DEFAULT))
+    ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--reps", type=int, default=5)
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("fftbench needs a CUDA device")
+    torch.cuda.set_device(0)
+    card = _card()
+    for spec in args.cases:
+        run_case(spec, args.warmup, args.reps, card)
+
+
+if __name__ == "__main__":
+    main()
