@@ -178,14 +178,6 @@ int nbk_fft_lines(void *cplx, int dtype, int64_t n_line, int64_t line_stride, in
 int nbk_fft_lines_oop(const void *src, void *dst, int dtype, int64_t n_line, int64_t line_stride, int64_t n_inner,
                       int64_t n_outer, int64_t outer_stride, int inverse, double scale, void *stream);
 int nbk_fft_z_forward(const void *real, void *cplx, int dtype, int64_t rows, int64_t Nz, void *stream);
-/* Fused line pass + slab transpose over NVLink peer memory: FFT along the second stored axis of the local slab
- * src[n_outer][n_line][n_inner]; output frequency k is stored directly into rank (k / (n_line/P))'s buffer at
- * peer[p][((k % (n_line/P)) * (n_outer*P) + outer_start + outer) * n_inner + kz].  peer_ptrs_host: host array of P
- * device pointers valid on this GPU (CUDA IPC / symmetric memory; entry `rank` = the local buffer).  Replaces
- * y-pass write + nbk_transpose_pack + all-to-all + nbk_transpose_unpack by one kernel; the caller provides the
- * cross-rank barriers before and after. */
-int nbk_fft_lines_scatter(const void *src, void *const *peer_ptrs_host, int dtype, int64_t n_line, int64_t n_inner,
-                          int64_t n_outer, int64_t outer_start, int P, int inverse, double scale, void *stream);
 int nbk_transpose_pack(const void *src, void *dst, int dtype, int64_t x_n, int64_t Ny, int64_t Nzc,
                        int64_t P, void *stream);
 int nbk_transpose_unpack(const void *src, void *dst, int dtype, int64_t y_n, int64_t Nx,
@@ -271,16 +263,14 @@ int nbk_ylm_mul_complex_acc2(void *acc, void *acc_mirror, const void *c, int dty
 int nbk_hermitian_expand(const void *comp, void *full, int dtype, const int64_t *nmesh_host, void *stream);
 int nbk_hermitian_compress(const void *full, void *comp, int dtype, int64_t rows, int64_t Nz, void *stream);
 
-/* Slab transpose as a line pass into P contiguous local send blocks send[p][k % (N/P)][outer][inner] followed by one
- * strided bulk copy per peer (cudaMemcpy2DAsync over NVLink, rows of n_outer * n_inner elements): the alternative to
- * nbk_fft_lines_scatter's fine-grained remote stores for the pencil transpose of pfft (r2c / c2r, base/mesh.py:228,237).
- * nbk_slab_push: block p of `send` -> rank p's field [rows_per_peer][n_outer * P][n_inner] at offset outer_start. */
-int nbk_fft_lines_pack(const void *src, void *send, int dtype, int64_t n_line, int64_t n_inner, int64_t n_outer, int P,
-                       int inverse, double scale, void *stream);
-int nbk_slab_push(const void *send, void *const *peer_ptrs_host, int dtype, int64_t rows_per_peer, int64_t n_outer,
-                  int64_t n_inner, int64_t outer_start, int P, int rank, void *stream);
-/* the same two steps restricted to the outer sub-range [o0, o0 + o_cnt) of the slab (planes of x in r2c, base/mesh.py:237):
- * the caller pushes one part over NVLink on a second stream while the line pass of the next part runs */
+/* Slab transpose over NVLink peer memory for the pencil transpose of pfft (r2c / c2r, base/mesh.py:228,237): a line
+ * pass (FFT along the second stored axis of src[n_outer][n_line][n_inner]) into P contiguous local send blocks
+ * send[p][k % (N/P)][n_outer][inner], followed by one strided bulk copy per peer (cudaMemcpy2DAsync, rows of
+ * n_outer * n_inner elements).  nbk_slab_push_range: block p of `send` -> rank p's field
+ * [rows_per_peer][n_outer * P][n_inner] at offset outer_start; peer_ptrs_host: host array of P device pointers valid
+ * on this GPU (entry `rank` = the local buffer).  Both steps cover the outer sub-range [o0, o0 + o_cnt) of the slab
+ * (planes of x in r2c, base/mesh.py:237): the caller pushes one part on a second stream while the line pass of the
+ * next part runs; o0 = 0, o_cnt = n_outer is the whole slab.  The caller provides the cross-rank barriers. */
 int nbk_fft_lines_pack_range(const void *src, void *send, int dtype, int64_t n_line, int64_t n_inner, int64_t n_outer,
                              int64_t o0, int64_t o_cnt, int P, int inverse, double scale, void *stream);
 int nbk_slab_push_range(const void *send, void *const *peer_ptrs_host, int dtype, int64_t rows_per_peer, int64_t n_outer,

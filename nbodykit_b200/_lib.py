@@ -53,7 +53,6 @@ SIGNATURES = {
     "nbk_fft_lines": ([_vp, _i, _i64, _i64, _i64, _i64, _i64, _i, _d, _vp], _i),
     "nbk_fft_lines_oop": ([_vp, _vp, _i, _i64, _i64, _i64, _i64, _i64, _i, _d, _vp], _i),
     "nbk_fft_z_forward": ([_vp, _vp, _i, _i64, _i64, _vp], _i),
-    "nbk_fft_lines_scatter": ([_vp, ctypes.POINTER(ctypes.c_void_p), _i, _i64, _i64, _i64, _i64, _i, _i, _d, _vp], _i),
     "nbk_transpose_pack": ([_vp, _vp, _i, _i64, _i64, _i64, _i64, _vp], _i),
     "nbk_transpose_unpack": ([_vp, _vp, _i, _i64, _i64, _i64, _i64, _vp], _i),
     "nbk_transpose_pack_back": ([_vp, _vp, _i, _i64, _i64, _i64, _i64, _vp], _i),
@@ -68,8 +67,6 @@ SIGNATURES = {
     "nbk_hermitian_expand": ([_vp, _vp, _i, _pi64, _vp], _i),
     "nbk_hermitian_compress": ([_vp, _vp, _i, _i64, _i64, _vp], _i),
     "nbk_resample_complex": ([_vp, _vp, _i, _pi64, _pi64, _vp], _i),
-    "nbk_fft_lines_pack": ([_vp, _vp, _i, _i64, _i64, _i64, _i, _i, _d, _vp], _i),
-    "nbk_slab_push": ([_vp, ctypes.POINTER(ctypes.c_void_p), _i, _i64, _i64, _i64, _i64, _i, _i, _vp], _i),
     "nbk_fft_lines_pack_range": ([_vp, _vp, _i, _i64, _i64, _i64, _i64, _i64, _i, _i, _d, _vp], _i),
     "nbk_slab_push_range": ([_vp, ctypes.POINTER(ctypes.c_void_p), _i, _i64, _i64, _i64, _i64, _i64, _i64, _i, _i, _vp], _i),
     "nbk_ylm_mul_real": ([_vp, _vp, _i, _i, _i, _pi64, _pd, _pd, _i64, _i64, _vp], _i),

@@ -701,9 +701,7 @@ static int launch_bin(const void *c1, const void *c2, const BinParams &P, const 
                                                                 (unsigned long long *)nsum, xsum, musum, ysum, kmin, \
                                                                 inv_dk, uniform, ct0, ct1, ctz);                      \
     } while (0)
-    static int lean_knob = -1;
-    if (lean_knob < 0) { const char *e = getenv("NBK_BIN_LEAN"); lean_knob = (e && e[0] == '0') ? 0 : 1; }   // 0: always the general kernel
-    const bool lean = lean_knob && smem_acc && !P.is_p3d && !P.has_c2 && P.c3 == nullptr && P.estride == 2 && P.coord_mode == 4 &&
+    const bool lean = smem_acc && !P.is_p3d && !P.has_c2 && P.c3 == nullptr && P.estride == 2 && P.coord_mode == 4 &&
                       P.hermitian == 1 && P.anti == 0;
     if (lean) { if (sym) LAUNCH_BIN(true, true, true); else LAUNCH_BIN(true, false, true); }
     else if (smem_acc) { if (sym) LAUNCH_BIN(true, true, false); else LAUNCH_BIN(true, false, false); }

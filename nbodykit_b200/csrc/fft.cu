@@ -10,10 +10,10 @@
 //   k_fft_lines_tma   lines of 256 / 512 / 1024: row groups stream through a ring of shared-memory slots as 4-D tensor-map
 //                     boxes (cp.async.bulk.tensor + mbarrier), one 64-point FFT per warp, one radix-R combine per tile
 //   k_fft_z_r2c_tma   rows of 256 / 512 / 1024 reals: warp-per-row, private ring of row buffers filled by 1-D bulk copies
-// Older families, still serving short lines, c8 lines whose rows are not 16-byte aligned, the backward z pass and the
-// NBK_FFT_LINES=rg|smem knob: the register-I/O kernels (k_fft_lines_rg, k_fft_z_r2c_rg: first radix-8 stage straight from
+// Older families, still serving the other lengths, c8 lines whose rows are not 16-byte aligned and the backward z pass:
+// the register-I/O kernels for lines of 64 and more (k_fft_lines_rg, k_fft_z_r2c_rg: first radix-8 stage straight from
 // global memory, last stage straight to the digit-reversed frequency rows, [N][B+1] padded tiles in between) and the
-// shared-memory kernels (k_fft_lines with cp.async double buffering, k_fft_z_r2c, k_fft_z_c2r).
+// shared-memory kernels (k_fft_lines with cp.async double buffering for lines below 64, k_fft_z_r2c, k_fft_z_c2r).
 // Decimation-in-frequency radix-8 butterflies in registers throughout (+ one radix-4 / radix-2 stage for the remainder of
 // log2 N).  Twiddles: f8-accurate table built on the device with sincospi, staged in shared memory.  Sizes: 2^k.
 // Sides that are products of 2, 3, 5 and 7 (Nx, Ny <= 4096; Nz <= 8192 even, <= 4095 odd) go through the separate
@@ -597,11 +597,6 @@ __device__ __forceinline__ void fm_tma_load_4d(void *sdst, const CUtensorMap *tm
                  :: "r"(fm_smem_u32(sdst)), "l"(tmap), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(fm_smem_u32(bar)) : "memory");
 }
 
-__device__ __forceinline__ void fm_tma_prefetch_4d(const CUtensorMap *tmap, int c0, int c1, int c2, int c3) {
-    asm volatile("cp.async.bulk.prefetch.tensor.4d.L2.global.tile [%0, {%1, %2, %3, %4}];"
-                 :: "l"(tmap), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-
 template <typename C> struct W16c;      // cos(pi/8), sin(pi/8)
 template <> struct W16c<float2> { static __device__ __forceinline__ float c() { return 0.92387953251128675613f; }
                                   static __device__ __forceinline__ float s() { return 0.38268343236508977173f; } };
@@ -643,14 +638,18 @@ template <int R, typename C> __device__ __forceinline__ void dftR(C (&a)[R]) {
     else { static_assert(R == 4, "combine radix"); dft4(a[0], a[1], a[2], a[3]); }
 }
 
+// CTAs of k_fft_lines_tma per SM, which its shared-memory ring is sized for (2; 3 at N = 256; the tile at N = 1024 takes
+// the whole SM).  Also its launch bound: without it ptxas trades spills for an occupancy the ring rules out.
+__host__ __device__ constexpr int tma_ctas_per_sm(int R) { return R == 16 ? 1 : R == 4 ? 3 : 2; }
+
 template <typename T, int R, int B, int NT, bool PEER>
-__global__ void __launch_bounds__(NT)
+__global__ void __launch_bounds__(NT, tma_ctas_per_sm(R))
 k_fft_lines_tma(const __grid_constant__ CUtensorMap tmap, typename C2<T>::type *dst, PeerPtrs<typename C2<T>::type> peers,
                 const typename C2<T>::type *__restrict__ twg, int64_t line_stride, int64_t n_inner, int64_t tiles_inner,
                 int64_t n_tiles, int64_t outer_stride, int n_per, int64_t d_total, int64_t outer_start, int inverse, T scale,
-                int NS, int l2_ahead) {
+                int NS) {
     typedef typename C2<T>::type C;
-    // B side-by-side lines: 128-byte rows (8 c16 / 16 c8), or 64-byte rows at N = 1024 so that TWO CTAs share an SM
+    // B side-by-side lines: 128-byte rows (8 c16 / 16 c8)
     constexpr int S = 64, N = S * R, NW = NT / 32, SLOT = S * B;
     static_assert((8 * B) % 32 == 0 && R % NW == 0, "tile geometry");
     extern __shared__ __align__(1024) unsigned char smem_raw[];
@@ -680,22 +679,9 @@ k_fft_lines_tma(const __grid_constant__ CUtensorMap tmap, typename C2<T>::type *
         fm_mbar_expect_tx(&bars[slot], (unsigned)(SLOT * sizeof(C)));
         fm_tma_load_4d(ring + (size_t)slot * SLOT, &tmap, (int)(2 * inner0), j, 0, (int)outer, &bars[slot]);
     };
-    // optional (l2_ahead, off by default): L2 prefetch of the boxes one tile beyond what the ring can hold
-    int fetched = 0;
-    auto prefetch = [&](int g) {
-        const int it = g / R, j = g - it * R;
-        const int64_t tile = first + (int64_t)it * gridDim.x;
-        const int64_t outer = tile / tiles_inner;
-        const int64_t inner0 = (tile - outer * tiles_inner) * B;
-        fm_tma_prefetch_4d(&tmap, (int)(2 * inner0), j, 0, (int)outer);
-    };
     if (tid == 0) {
         const int upto = G < NS ? G : NS;
         for (; issued < upto; issued++) issue(issued);
-        if (l2_ahead) {
-            int pf = issued + R < G ? issued + R : G;
-            for (fetched = issued; fetched < pf; fetched++) prefetch(fetched);
-        }
     }
     for (int it = 0; it < my_tiles; it++) {
         const int64_t tile = first + (int64_t)it * gridDim.x;
@@ -770,11 +756,6 @@ k_fft_lines_tma(const __grid_constant__ CUtensorMap tmap, typename C2<T>::type *
             int upto = (it + 1) * R + NS;
             if (upto > G) upto = G;
             for (; issued < upto; issued++) issue(issued);
-            if (l2_ahead) {
-                int pf = issued + R < G ? issued + R : G;
-                if (fetched < issued) fetched = issued;
-                for (; fetched < pf; fetched++) prefetch(fetched);
-            }
         }
     }
 }
@@ -1231,33 +1212,16 @@ static int pick_B(int N, int csize, int64_t n_inner) {
     return B;
 }
 
-static bool use_reg_lines(int N) {
-    static int mode = -1;
-    if (mode < 0) {
-        const char *e = getenv("NBK_FFT_LINES");
-        mode = (e && strcmp(e, "smem") == 0) ? 0 : 1;      // "rg" / default: register-I/O family (the TMA pass is tried first)
-    }
-    return mode == 1 && N >= 64;
-}
-
 // TMA-pipelined line pass (k_fft_lines_tma) where it applies: N in {256, 512, 1024}, 16-byte aligned rows (always true
 // for c16 fields; c8 fields with an odd row length -- the y pass over Nz/2+1 columns -- keep the register-I/O kernel).
-// NBK_FFT_LINES=rg|smem selects the older kernels.  *done = false: not applicable, the caller falls back.
-static int lines_mode() {
-    static int mode = -1;
-    if (mode < 0) {
-        const char *e = getenv("NBK_FFT_LINES");
-        mode = (e && strcmp(e, "smem") == 0) ? 0 : (e && strcmp(e, "rg") == 0) ? 1 : 2;
-    }
-    return mode;
-}
+// *done = false: not applicable, the caller falls back.  d_total: rows of the peer field (peer stores only).
 template <typename T>
 static int launch_lines_tma(const void *src, void *dst, void *const *peer_host, int P, int N, int64_t line_stride,
                             int64_t n_inner, int64_t n_outer, int64_t outer_stride, int64_t outer_start, int inverse,
-                            double scale, cudaStream_t s, int64_t d_total_override, bool *done) {
+                            double scale, cudaStream_t s, int64_t d_total, bool *done) {
     typedef typename C2<T>::type C;
     *done = false;
-    if (lines_mode() != 2 || (N != 256 && N != 512 && N != 1024)) return NBK_OK;
+    if (N != 256 && N != 512 && N != 1024) return NBK_OK;
     const size_t cs = sizeof(C);
     if (n_outer > 1 && outer_stride == 0) return NBK_OK;
     const int64_t ostride = n_outer > 1 ? outer_stride : (int64_t)N * line_stride;
@@ -1267,17 +1231,7 @@ static int launch_lines_tma(const void *src, void *dst, void *const *peer_host, 
     nbk_encode_tiled_fn enc = get_tensor_map_encoder();
     if (!enc) return NBK_OK;
     const int R = N / 64;
-    // tile width: 128-byte rows.  (64-byte rows -- half the ring, two CTAs per SM at N = 1024 -- are selectable with
-    // NBK_FFT_TMA_B = columns.)
-    static int knob_b = -1, knob_ns = -1, l2_ahead = -1;
-    // NBK_FFT_TMA_L2=1: L2 tensor prefetch one tile ahead of the ring.  Off by default: the prefetches compete with the demand
-    // loads and stores for DRAM.
-    if (l2_ahead < 0) { const char *e = getenv("NBK_FFT_TMA_L2"); l2_ahead = (e && e[0] == '1') ? 1 : 0; }
-    if (knob_b < 0) { const char *e = getenv("NBK_FFT_TMA_B"); knob_b = e ? atoi(e) : 0; }
-    if (knob_ns < 0) { const char *e = getenv("NBK_FFT_TMA_NS"); knob_ns = e ? atoi(e) : 0; }
-    const int Bfull = 128 / (int)cs;
-    int B = Bfull;
-    if (N != 256 && (knob_b == Bfull || knob_b == Bfull / 2)) B = knob_b;
+    constexpr int B = 128 / (int)sizeof(C);                    // tile width: 128-byte rows
     CUtensorMap tmap;
     const cuuint64_t gdim[4] = {(cuuint64_t)(2 * n_inner), (cuuint64_t)R, 64, (cuuint64_t)n_outer};
     const cuuint64_t gstr[3] = {(cuuint64_t)line_stride * cs, (cuuint64_t)R * line_stride * cs, (cuuint64_t)ostride * cs};
@@ -1291,15 +1245,13 @@ static int launch_lines_tma(const void *src, void *dst, void *const *peer_host, 
     void *tw;
     int rc = get_twiddle(N, dtype, s, &tw);
     if (rc) return rc;
-    // ring: R slots of the tile being transformed + P prefetch slots, sized for 2 CTAs / SM (3 at N = 256); the wide
-    // tile at N = 1024 takes the whole SM
+    // ring: R slots of the tile being transformed + P prefetch slots, sized for tma_ctas_per_sm(R) CTAs per SM
     const size_t slot = (size_t)64 * B * cs;
     const size_t fixed = (size_t)(N + 64) * cs + 26 * 8 + 64;
-    int per_sm = (R == 16 && B == Bfull) ? 1 : (R == 4 ? 3 : 2);
+    const int per_sm = tma_ctas_per_sm(R);
     int NS = (int)(((size_t)(226 * 1024) / per_sm - 1024 - fixed) / slot);
     if (NS > 26) NS = 26;
     if (NS > 2 * R) NS = 2 * R;
-    if (knob_ns >= R + 1 && knob_ns <= NS) NS = knob_ns;
     NBK_CHECK_ARG(NS >= R + 1, "fft_lines: the slot ring does not fit in shared memory (N = %d)", N);
     const size_t smem = (size_t)NS * slot + fixed;
     const int64_t tiles_inner = (n_inner + B - 1) / B;
@@ -1308,20 +1260,16 @@ static int launch_lines_tma(const void *src, void *dst, void *const *peer_host, 
     PeerPtrs<C> peers;
     for (int i = 0; i < NBK_MAX_PEERS; i++) peers.p[i] = (peer_host && i < P) ? (C *)peer_host[i] : nullptr;
     const int n_per = peer_host ? N / P : N;
-    const int64_t d_total = d_total_override ? d_total_override : (peer_host ? n_outer * P : 0);
 #define LAUNCH_TMA2(RR, BB, NTT, PEERF)                                                                                \
     do {                                                                                                               \
         NBK_CUDA(cudaFuncSetAttribute(k_fft_lines_tma<T, RR, BB, NTT, PEERF>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
         k_fft_lines_tma<T, RR, BB, NTT, PEERF><<<(int)g, NTT, smem, s>>>(tmap, (C *)dst, peers, (const C *)tw, line_stride, n_inner, \
-            tiles_inner, n_tiles, outer_stride, n_per, d_total, outer_start, inverse, (T)scale, NS, l2_ahead);        \
+            tiles_inner, n_tiles, outer_stride, n_per, d_total, outer_start, inverse, (T)scale, NS);                  \
     } while (0)
 #define LAUNCH_TMA(RR, BB, NTT) do { if (peer_host) LAUNCH_TMA2(RR, BB, NTT, true); else LAUNCH_TMA2(RR, BB, NTT, false); } while (0)
-    constexpr int BF = 128 / (int)sizeof(C), BH = BF / 2;
-    if (R == 16 && B == BF) LAUNCH_TMA(16, BF, 512);
-    else if (R == 16) LAUNCH_TMA(16, BH, 256);
-    else if (R == 8 && B == BF) LAUNCH_TMA(8, BF, 256);
-    else if (R == 8) LAUNCH_TMA(8, BH, 256);
-    else LAUNCH_TMA(4, BF, 128);
+    if (R == 16) LAUNCH_TMA(16, B, 512);
+    else if (R == 8) LAUNCH_TMA(8, B, 256);
+    else LAUNCH_TMA(4, B, 128);
 #undef LAUNCH_TMA
 #undef LAUNCH_TMA2
     NBK_LAUNCHED();
@@ -1329,40 +1277,26 @@ static int launch_lines_tma(const void *src, void *dst, void *const *peer_host, 
     return NBK_OK;
 }
 
-// register-I/O line pass; peer_host != nullptr selects the peer-memory scatter store
+// register-I/O line pass (N >= 64; the TMA pass is tried first); peer_host != nullptr selects the peer-memory scatter
+// store into a field of d_total rows
 template <typename T>
 static int launch_lines_rg(const void *src, void *dst, void *const *peer_host, int P, int N, int64_t line_stride,
                            int64_t n_inner, int64_t n_outer, int64_t outer_stride, int64_t outer_start, int inverse,
-                           double scale, cudaStream_t s, int64_t d_total_override = 0) {
+                           double scale, cudaStream_t s, int64_t d_total) {
     typedef typename C2<T>::type C;
     {
         bool done = false;
         int rct = launch_lines_tma<T>(src, dst, peer_host, P, N, line_stride, n_inner, n_outer, outer_stride, outer_start,
-                                      inverse, scale, s, d_total_override, &done);
+                                      inverse, scale, s, d_total, &done);
         if (rct || done) return rct;
     }
     int dtype = sizeof(T) == 4 ? NBK_F4 : NBK_F8;
     void *tw;
     int rc = get_twiddle(N, dtype, s, &tw);
     if (rc) return rc;
-    // tile width: 128-byte runs; the peer-memory scatter uses 256-byte runs (wider NVLink writes; NBK_FFT_PEER_RUN=128 restores the narrow tile)
-    static int peer_run = -1;
-    if (peer_run < 0) {
-        const char *e = getenv("NBK_FFT_PEER_RUN");
-        peer_run = e ? atoi(e) : 256;
-        if (peer_run != 128 && peer_run != 256) peer_run = 256;
-    }
-    int B = (peer_host ? peer_run : 128) / (int)sizeof(C);
+    // tile width: 128-byte runs; the peer-memory scatter uses 256-byte runs (wider NVLink writes)
+    int B = (peer_host ? 256 : 128) / (int)sizeof(C);
     if (B > 16) B = 16;
-    // experiment knobs: NBK_FFT_LINE_B (tile width), NBK_FFT_LINE_NT (threads per CTA: 128 / 256 / 512)
-    static int knob_b = -1, knob_nt = -1;
-    if (knob_b < 0) {
-        const char *e = getenv("NBK_FFT_LINE_B");
-        knob_b = e ? atoi(e) : 0;
-        e = getenv("NBK_FFT_LINE_NT");
-        knob_nt = e ? atoi(e) : 0;
-    }
-    if (!peer_host && (knob_b == 2 || knob_b == 4 || knob_b == 8 || knob_b == 16)) B = knob_b;
     while (B > 1 && ((size_t)N * (B + 2) * sizeof(C) > 220 * 1024 || B / 2 >= n_inner)) B >>= 1;
     size_t smem = (size_t)N * (B + 2) * sizeof(C);
     NBK_CHECK_ARG(smem <= 227 * 1024, "fft_lines: N=%d does not fit in shared memory", N);
@@ -1371,22 +1305,12 @@ static int launch_lines_rg(const void *src, void *dst, void *const *peer_host, i
     int per_sm = (int)((227 * 1024) / (smem + 1024));
     if (per_sm < 1) per_sm = 1;
     if (per_sm > 4) per_sm = 4;
-    int nthreads = (per_sm == 1 && B >= 4) ? 512 : 256;
-    if (!peer_host && knob_nt == 128 && B >= 2 && B <= 8) nthreads = 128;
-    if (!peer_host && knob_nt == 512 && B >= 4) nthreads = 512;
-    if (nthreads == 128 && per_sm > 4) per_sm = 4;
+    const int nthreads = (per_sm == 1 && B >= 4) ? 512 : 256;
     if (nthreads == 256 && per_sm > 2) per_sm = 2;       // 128 registers per thread
-    if (nthreads == 512) per_sm = 1;
     int64_t g = n_tiles < (int64_t)NBK_SM_COUNT * per_sm ? n_tiles : (int64_t)NBK_SM_COUNT * per_sm;
     PeerPtrs<C> peers;
     for (int i = 0; i < NBK_MAX_PEERS; i++) peers.p[i] = (peer_host && i < P) ? (C *)peer_host[i] : nullptr;
     const int n_per = peer_host ? N / P : N;
-    const int64_t d_total = d_total_override ? d_total_override : (peer_host ? n_outer * P : 0);
-    static int prefetch = -1;
-    if (prefetch < 0) {
-        const char *e = getenv("NBK_FFT_PREFETCH");
-        prefetch = (e && e[0] == '0') ? 0 : 1;
-    }
     const int first_per_thread = (int)(((int64_t)(N >> 3) * B) / nthreads);
     const bool exact = ((int64_t)(N >> 3) * B) % nthreads == 0;
 #define LAUNCH_RGP(BB, NTT, IT)                                                                                       \
@@ -1400,7 +1324,7 @@ static int launch_lines_rg(const void *src, void *dst, void *const *peer_host, i
                 ilog2(N), line_stride, n_inner, tiles_inner, n_tiles, outer_stride, n_per, d_total, outer_start, inverse, (T)scale); \
         }
     // the common shapes: two first-stage butterflies per thread (512^3: B=8/16, 256 threads; 1024^3: B=8, 512 threads)
-    if (prefetch && exact && first_per_thread == 2) {
+    if (exact && first_per_thread == 2) {
         bool done = true;
         if (nthreads == 512 && B == 8) { LAUNCH_RGP(8, 512, 2) }
         else if (nthreads == 512 && B == 16) { LAUNCH_RGP(16, 512, 2) }
@@ -1422,12 +1346,7 @@ static int launch_lines_rg(const void *src, void *dst, void *const *peer_host, i
                 ilog2(N), line_stride, n_inner, tiles_inner, n_tiles, outer_stride, n_per, d_total, outer_start, inverse, (T)scale); \
         }                                                                                                          \
         break;
-    if (nthreads == 128) {
-        switch (B) {
-            LAUNCH_RG(2, 128) LAUNCH_RG(4, 128) LAUNCH_RG(8, 128)
-            default: nbk_set_error("fft_lines: internal tile width %d", B); return NBK_ERR_ARG;
-        }
-    } else if (nthreads == 512) {
+    if (nthreads == 512) {
         switch (B) {
             LAUNCH_RG(4, 512) LAUNCH_RG(8, 512) LAUNCH_RG(16, 512)
             default: nbk_set_error("fft_lines: internal tile width %d", B); return NBK_ERR_ARG;
@@ -1455,8 +1374,8 @@ static int launch_lines(const void *data, void *dst, int N, int64_t line_stride,
         }
         return NBK_OK;
     }
-    if (use_reg_lines(N))
-        return launch_lines_rg<T>(data, dst, nullptr, 1, N, line_stride, n_inner, n_outer, outer_stride, 0, inverse, scale, s);
+    if (N >= 64)
+        return launch_lines_rg<T>(data, dst, nullptr, 1, N, line_stride, n_inner, n_outer, outer_stride, 0, inverse, scale, s, 0);
     void *tw;
     int rc = get_twiddle(N, dtype, s, &tw);
     if (rc) return rc;
@@ -1514,13 +1433,13 @@ extern "C" int nbk_fft_lines_oop(const void *src, void *dst, int dtype, int64_t 
     return launch_lines<double>(src, dst, (int)n_line, line_stride, n_inner, n_outer, outer_stride, inverse, scale, s);
 }
 
+// line pass whose output rows go to the P blocks of peer_host, each a field of d_total rows [N/P][d_total][n_inner]
 template <typename T>
 static int launch_lines_scatter(const void *src, void *const *peer_host, int N, int64_t n_inner, int64_t n_outer,
-                                int64_t outer_start, int P, int inverse, double scale, cudaStream_t s,
-                                int64_t d_total_override = 0) {
-    if (use_reg_lines(N))
+                                int64_t outer_start, int P, int inverse, double scale, cudaStream_t s, int64_t d_total) {
+    if (N >= 64)
         return launch_lines_rg<T>(src, nullptr, peer_host, P, N, n_inner, n_inner, n_outer, (int64_t)N * n_inner, outer_start,
-                                  inverse, scale, s, d_total_override);
+                                  inverse, scale, s, d_total);
     typedef typename C2<T>::type C;
     int dtype = sizeof(T) == 4 ? NBK_F4 : NBK_F8;
     void *tw;
@@ -1541,8 +1460,7 @@ static int launch_lines_scatter(const void *src, void *const *peer_host, int N, 
     case BB:                                                                                                         \
         NBK_CUDA(cudaFuncSetAttribute(k_fft_lines_scatter<T, BB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
         k_fft_lines_scatter<T, BB><<<(int)g, 256, smem, s>>>((const C *)src, peers, (const C *)tw, N, ilog2(N), n_inner, \
-                                                             tiles_inner, n_tiles, N / P,                              \
-                                                             d_total_override ? d_total_override : n_outer * P, outer_start, \
+                                                             tiles_inner, n_tiles, N / P, d_total, outer_start,      \
                                                              inverse, (T)scale);                                     \
         break;
     switch (B) {
@@ -1552,19 +1470,6 @@ static int launch_lines_scatter(const void *src, void *const *peer_host, int N, 
 #undef LAUNCH_LS
     NBK_LAUNCHED();
     return NBK_OK;
-}
-
-extern "C" int nbk_fft_lines_scatter(const void *src, void *const *peer_ptrs_host, int dtype, int64_t n_line,
-                                     int64_t n_inner, int64_t n_outer, int64_t outer_start, int P, int inverse,
-                                     double scale, void *stream) {
-    NBK_CHECK_ARG(dtype == NBK_F4 || dtype == NBK_F8, "fft_lines_scatter: bad dtype %d", dtype);
-    NBK_CHECK_ARG(is_pow2(n_line) && n_line >= 2 && n_line <= 8192, "fft_lines_scatter: line length %lld unsupported", (long long)n_line);
-    NBK_CHECK_ARG(P >= 1 && P <= NBK_MAX_PEERS && n_line % P == 0, "fft_lines_scatter: bad peer count %d", P);
-    if (n_inner <= 0 || n_outer <= 0) return NBK_OK;
-    cudaStream_t s = (cudaStream_t)stream;
-    if (dtype == NBK_F4)
-        return launch_lines_scatter<float>(src, peer_ptrs_host, (int)n_line, n_inner, n_outer, outer_start, P, inverse, scale, s);
-    return launch_lines_scatter<double>(src, peer_ptrs_host, (int)n_line, n_inner, n_outer, outer_start, P, inverse, scale, s);
 }
 
 template <typename T>
@@ -1577,7 +1482,7 @@ static int launch_z(const void *in, void *out, int64_t rows, int Nz, bool forwar
     if (rc) return rc;
     rc = get_twiddle(Nz, dtype, s, &twN);
     if (rc) return rc;
-    if (forward && lines_mode() == 2 && (M == 128 || M == 256 || M == 512) && (reinterpret_cast<uintptr_t>(in) & 15) == 0 &&
+    if (forward && (M == 128 || M == 256 || M == 512) && (reinterpret_cast<uintptr_t>(in) & 15) == 0 &&
         ((size_t)Nz * sizeof(T)) % 16 == 0) {
         // warp-per-row TMA pass: 12 warps, per-warp ring of row buffers filling the SM's shared memory
         constexpr int NWZ = 12;
@@ -1586,9 +1491,6 @@ static int launch_z(const void *in, void *out, int64_t rows, int Nz, bool forwar
         int nbuf = (int)(((size_t)224 * 1024 - twb - 1024) / (NWZ * rowb));
         if (nbuf > 4) nbuf = 4;
         if (nbuf < 2) nbuf = 2;
-        static int knob_nb = -1;
-        if (knob_nb < 0) { const char *e = getenv("NBK_FFT_Z_NBUF"); knob_nb = e ? atoi(e) : 0; }
-        if (knob_nb >= 1 && knob_nb <= nbuf) nbuf = knob_nb;
         const size_t smem = twb + (size_t)NWZ * nbuf * rowb + (size_t)NWZ * nbuf * 8 + 128;
         NBK_CHECK_ARG(smem <= 227 * 1024, "fft z pass: Nz=%d does not fit in shared memory", Nz);
         int64_t g = (rows + NWZ - 1) / NWZ;
@@ -1603,7 +1505,7 @@ static int launch_z(const void *in, void *out, int64_t rows, int Nz, bool forwar
         NBK_LAUNCHED();
         return NBK_OK;
     }
-    if (forward && M >= 64 && M <= 256 * (sizeof(T) == 4 ? 16 : 8) && use_reg_lines(M)) {   // the tile must fit the registers
+    if (forward && M >= 64 && M <= 256 * (sizeof(T) == 4 ? 16 : 8)) {   // the tile must fit the registers
         // register-I/O variant: 256 threads hold the whole tile across the last stage (M * B <= 256 V)
         const int V = sizeof(T) == 4 ? 16 : 8;
         int B = 16;
@@ -1921,28 +1823,12 @@ extern "C" int nbk_resample_complex(const void *src, void *dst, int dtype, const
 // Slab transpose as "line pass into send blocks" + bulk peer copies (P > 1).  The line pass (y pass of r2c, inverse x
 // pass of c2r) stores its output rows directly in transposed order into P contiguous LOCAL blocks
 //     send[p][kl][outer][inner]      kl = k % (N/P) the line frequency inside rank p's share, outer < n_outer
-// and nbk_slab_push() moves block p into rank p's field [N/P][n_outer * P][n_inner] with one strided bulk copy per
+// and nbk_slab_push_range() moves block p into rank p's field [N/P][n_outer * P][n_inner] with one strided bulk copy per
 // peer: rows of n_outer * n_inner contiguous elements (1 MB at 1024^3 on 8 GPUs) travel over NVLink on the copy
-// engines at link rate, instead of the 128..256-byte remote stores of nbk_fft_lines_scatter.
+// engines at link rate, instead of 128..256-byte remote stores from the line pass.
+// Both work on the outer sub-range [o0, o0 + o_cnt) of the slab (the send blocks keep their full [kl][n_outer][inner]
+// shape): the caller pushes one part of the slab while the next part is still being transformed.
 // ---------------------------------------------------------------------------------------------
-extern "C" int nbk_fft_lines_pack(const void *src, void *send, int dtype, int64_t n_line, int64_t n_inner, int64_t n_outer,
-                                  int P, int inverse, double scale, void *stream) {
-    NBK_CHECK_ARG(dtype == NBK_F4 || dtype == NBK_F8, "fft_lines_pack: bad dtype %d", dtype);
-    NBK_CHECK_ARG(is_pow2(n_line) && n_line >= 2 && n_line <= 8192, "fft_lines_pack: line length %lld unsupported", (long long)n_line);
-    NBK_CHECK_ARG(P >= 1 && P <= NBK_MAX_PEERS && n_line % P == 0, "fft_lines_pack: bad peer count %d", P);
-    if (n_inner <= 0 || n_outer <= 0) return NBK_OK;
-    const size_t cs = dtype == NBK_F4 ? 8 : 16;
-    const size_t block = (size_t)(n_line / P) * n_outer * n_inner * cs;
-    void *blocks[NBK_MAX_PEERS];
-    for (int p = 0; p < P; p++) blocks[p] = (char *)send + (size_t)p * block;
-    cudaStream_t s = (cudaStream_t)stream;
-    if (dtype == NBK_F4)
-        return launch_lines_scatter<float>(src, blocks, (int)n_line, n_inner, n_outer, 0, P, inverse, scale, s, n_outer);
-    return launch_lines_scatter<double>(src, blocks, (int)n_line, n_inner, n_outer, 0, P, inverse, scale, s, n_outer);
-}
-
-// the same line pass restricted to the outer sub-range [o0, o0 + o_cnt) of the slab (the send blocks keep their full
-// [kl][n_outer][inner] shape): lets the caller push one part of the slab while the next part is still being transformed
 extern "C" int nbk_fft_lines_pack_range(const void *src, void *send, int dtype, int64_t n_line, int64_t n_inner,
                                         int64_t n_outer, int64_t o0, int64_t o_cnt, int P, int inverse, double scale,
                                         void *stream) {
@@ -1962,7 +1848,6 @@ extern "C" int nbk_fft_lines_pack_range(const void *src, void *send, int dtype, 
     return launch_lines_scatter<double>(sub, blocks, (int)n_line, n_inner, o_cnt, o0, P, inverse, scale, s, n_outer);
 }
 
-// nbk_slab_push for the outer sub-range [o0, o0 + o_cnt) of every row
 extern "C" int nbk_slab_push_range(const void *send, void *const *peer_ptrs_host, int dtype, int64_t rows_per_peer,
                                    int64_t n_outer, int64_t n_inner, int64_t outer_start, int64_t o0, int64_t o_cnt, int P,
                                    int rank, void *stream) {
@@ -1980,24 +1865,6 @@ extern "C" int nbk_slab_push_range(const void *send, void *const *peer_ptrs_host
         const char *srcp = (const char *)send + (size_t)p * rows_per_peer * spitch + (size_t)o0 * n_inner * cs;
         char *dstp = (char *)peer_ptrs_host[p] + (size_t)(outer_start + o0) * n_inner * cs;
         NBK_CUDA(cudaMemcpy2DAsync(dstp, dpitch, srcp, spitch, width, (size_t)rows_per_peer, cudaMemcpyDeviceToDevice, s));
-    }
-    return NBK_OK;
-}
-
-extern "C" int nbk_slab_push(const void *send, void *const *peer_ptrs_host, int dtype, int64_t rows_per_peer,
-                             int64_t n_outer, int64_t n_inner, int64_t outer_start, int P, int rank, void *stream) {
-    NBK_CHECK_ARG(dtype == NBK_F4 || dtype == NBK_F8, "slab_push: bad dtype %d", dtype);
-    NBK_CHECK_ARG(P >= 1 && P <= NBK_MAX_PEERS && rank >= 0 && rank < P, "slab_push: bad peer count / rank");
-    if (rows_per_peer <= 0 || n_outer <= 0 || n_inner <= 0) return NBK_OK;
-    const size_t cs = dtype == NBK_F4 ? 8 : 16;
-    const size_t width = (size_t)n_outer * n_inner * cs;            // one kl row of my block
-    const size_t dpitch = width * P;                                // the same row of the destination field
-    cudaStream_t s = (cudaStream_t)stream;
-    for (int i = 0; i < P; i++) {
-        const int p = (rank + i) % P;                               // every rank starts with a different peer
-        const char *srcp = (const char *)send + (size_t)p * rows_per_peer * width;
-        char *dstp = (char *)peer_ptrs_host[p] + (size_t)outer_start * n_inner * cs;
-        NBK_CUDA(cudaMemcpy2DAsync(dstp, dpitch, srcp, width, width, (size_t)rows_per_peer, cudaMemcpyDeviceToDevice, s));
     }
     return NBK_OK;
 }

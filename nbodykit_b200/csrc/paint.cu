@@ -535,30 +535,6 @@ __device__ __forceinline__ void quad_claim(unsigned *hist, const int (&k)[4], un
     }
 }
 
-// ---- TMA bulk copy global -> shared with an mbarrier (1-D: no tensor map needed)
-__device__ __forceinline__ unsigned smem_u32(const void *p) { return (unsigned)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t *bar, unsigned count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, unsigned bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void *sdst, const void *gsrc, unsigned bytes, uint64_t *bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 :: "r"(smem_u32(sdst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, unsigned parity) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "NBK_WAIT:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra NBK_DONE;\n"
-        "bra NBK_WAIT;\n"
-        "NBK_DONE:\n"
-        "}\n" :: "r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-
 // workspace header words
 enum { HDR_QUEUE = 0, HDR_ABSMAX = 1, HDR_MODE = 2, HDR_DEFER = 3, HDR_WORDS = 64 };
 
@@ -567,8 +543,6 @@ struct BucketPlan {          // one bucketing configuration (host side, by value
     int W;                   // tile window (entries of the shared histogram)
     int nchunks;             // particle chunks (CTAs loop over them)
     int64_t chunk;           // particles per chunk, multiple of 4
-    int staged;              // particle coordinates staged by TMA bulk copies (needs a 16-byte aligned array)
-    int nst;                 // slots of the staging ring
     int wstage;              // scatter pass: records leave through a per-warp shared-memory transposition (coalesced stores)
     int stage_off;           // ... byte offset of the warps' staging areas in dynamic shared memory
 };
@@ -597,18 +571,7 @@ k_bucket_probe(const PT *__restrict__ pos, int64_t n, TileGeom tg, unsigned *__r
     if (threadIdx.x == 0) hdr[HDR_MODE] = (s_tot > 0 && 4 * s_ok >= 3 * s_tot) ? 1u : 0u;
 }
 
-// quad of this thread from the staged chunk (shared memory) or straight from global memory
-template <typename PT>
-__device__ __forceinline__ void load_quad_smem(const PT *sbuf, PT (&x)[4][3]) {
-    constexpr int NV = (int)(12 * sizeof(PT) / 16);
-    const uint4 *v = reinterpret_cast<const uint4 *>(sbuf + 12 * threadIdx.x);
-    uint4 r[NV];
-#pragma unroll
-    for (int k = 0; k < NV; k++) r[k] = v[k];
-    const PT *f = reinterpret_cast<const PT *>(r);
-#pragma unroll
-    for (int u = 0; u < 4; u++) { x[u][0] = f[3 * u]; x[u][1] = f[3 * u + 1]; x[u][2] = f[3 * u + 2]; }
-}
+// quad of this thread, straight from global memory
 template <typename PT>
 __device__ __forceinline__ void load_quad_gmem(const PT *__restrict__ cpos, int j0, int nv, bool aligned, PT (&x)[4][3]) {
     if (aligned && nv == 4) {
@@ -636,45 +599,19 @@ __device__ __forceinline__ double load_mass(const void *mass, int mass_f4, int64
 }
 
 // The chunk loop shared by the count and the scatter pass.  Rounds of 4 * blockDim particles: every thread owns one
-// aligned quad per round.  STAGED: thread 0 keeps nst - 1 rounds in flight as TMA bulk copies into a shared-memory
-// ring of nst slots (full rounds only; the ragged tail of the last chunk is read directly).  `body(j0, nv, x)` is
-// called by ALL threads (nv = 0 for idle ones) so that it may use warp collectives.
-template <typename PT, bool STAGED, typename F>
-__device__ __forceinline__ void chunk_rounds(const PT *__restrict__ cpos, int cn, PT *sring, uint64_t *bars, int nst,
-                                             unsigned &seq, bool aligned, F body) {
+// aligned quad per round.  `body(j0, nv, x)` is called by ALL threads (nv = 0 for idle ones) so that it may use warp
+// collectives.
+template <typename PT, typename F>
+__device__ __forceinline__ void chunk_rounds(const PT *__restrict__ cpos, int cn, bool aligned, F body) {
     const int SP = 4 * (int)blockDim.x;                       // particles per round
     const int nround = (cn + SP - 1) / SP;
-    const unsigned rbytes = (unsigned)(SP * 3 * sizeof(PT));
-    const int nfull = STAGED ? cn / SP : 0;                   // rounds that are copied whole
-    if (STAGED && threadIdx.x == 0) {
-        for (int s = 0; s < nst && s < nfull; s++) {
-            const unsigned slot = (seq + s) % (unsigned)nst;
-            mbar_expect_tx(&bars[slot], rbytes);
-            bulk_g2s(sring + (size_t)slot * SP * 3, cpos + (size_t)s * SP * 3, rbytes, &bars[slot]);
-        }
-    }
     for (int s = 0; s < nround; s++) {
         const int j0 = s * SP + 4 * (int)threadIdx.x;
         const int nv = min(4, max(0, cn - j0));
         PT x[4][3];
-        if (STAGED && s < nfull) {
-            const unsigned q = seq + s, slot = q % (unsigned)nst;
-            mbar_wait(&bars[slot], (q / (unsigned)nst) & 1);
-            load_quad_smem(sring + (size_t)slot * SP * 3, x);
-        } else {
-            load_quad_gmem(cpos, j0, nv, aligned, x);
-        }
+        load_quad_gmem(cpos, j0, nv, aligned, x);
         body(j0, nv, x);
-        if (STAGED && s < nfull) {
-            __syncthreads();                                   // every thread has read this ring slot
-            if (threadIdx.x == 0 && s + nst < nfull) {
-                const unsigned slot = (seq + s + nst) % (unsigned)nst;
-                mbar_expect_tx(&bars[slot], rbytes);
-                bulk_g2s(sring + (size_t)slot * SP * 3, cpos + (size_t)(s + nst) * SP * 3, rbytes, &bars[slot]);
-            }
-        }
     }
-    if (STAGED) seq += (unsigned)nfull;
 }
 
 // exact tile ids of a quad (fast float32 path, exact recomputation where it is not decisive)
@@ -723,7 +660,7 @@ __device__ __forceinline__ int chunk_window_lo(const PT *__restrict__ cpos, int 
 
 // MAXT: 512 (coherent plan: three CTAs per SM -- the register cap that goes with it is what keeps the count pass at 40
 // registers) or 1024 (scattered plan: one CTA per SM around a 200 KB histogram)
-template <int SUP, typename PT, bool STAGED, int MAXT>
+template <int SUP, typename PT, int MAXT>
 __global__ void __launch_bounds__(MAXT, MAXT == 512 ? 3 : 1)
 k_bucket_count(const PT *__restrict__ pos, const void *__restrict__ mass, int mass_f4, int64_t n, TileGeom tg, FastTile ft,
                unsigned *__restrict__ hdr, unsigned *__restrict__ cnt_w, unsigned *__restrict__ cnt_o,
@@ -731,15 +668,8 @@ k_bucket_count(const PT *__restrict__ pos, const void *__restrict__ mass, int ma
     if ((int)hdr[HDR_MODE] != bp.mode) return;
     extern __shared__ __align__(128) unsigned char s_raw[];
     unsigned *s_hist = reinterpret_cast<unsigned *>(s_raw);
-    PT *sring = reinterpret_cast<PT *>(s_raw + (((size_t)bp.W * sizeof(unsigned) + 127) & ~(size_t)127));
-    __shared__ uint64_t bars[8];
     __shared__ int s_lo;
-    if (STAGED && threadIdx.x == 0) {
-        for (int i = 0; i < 8; i++) mbar_init(&bars[i], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
     const bool aligned = (reinterpret_cast<uintptr_t>(pos) & 15) == 0;
-    unsigned seq = 0;
     float mx = 0.f;
     for (int c = blockIdx.x; c < bp.nchunks; c += gridDim.x) {
         const int64_t b = (int64_t)c * bp.chunk;
@@ -750,7 +680,7 @@ k_bucket_count(const PT *__restrict__ pos, const void *__restrict__ mass, int ma
         __syncthreads();
         const int lo = chunk_window_lo<SUP, PT>(cpos, cn, tg, bp.W, &s_lo);
         if (threadIdx.x == 0) win_lo[c] = lo;
-        chunk_rounds<PT, STAGED>(cpos, cn, sring, bars, bp.nst, seq, aligned, [&](int j0, int nv, const PT (&x)[4][3]) {
+        chunk_rounds<PT>(cpos, cn, aligned, [&](int j0, int nv, const PT (&x)[4][3]) {
             int t[4], k[4];
             quad_tiles<SUP, PT>(x, nv, tg, ft, t);
             bool anyout = false;
@@ -867,7 +797,7 @@ k_tile_scan(const unsigned *__restrict__ cnt_w, const unsigned *__restrict__ cnt
     if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) { offsets[ntiles] = carry + warp_tot[31]; hdr[HDR_QUEUE] = 0; }
 }
 
-template <int SUP, typename PT, bool STAGED, int MAXT>
+template <int SUP, typename PT, int MAXT>
 __global__ void __launch_bounds__(MAXT, MAXT == 512 ? 2 : 1)
 k_bucket_scatter(const PT *__restrict__ pos, const void *__restrict__ mass, int mass_f4, int64_t n, TileGeom tg, FastTile ft,
                  const unsigned *__restrict__ hdr, const unsigned *__restrict__ offsets,
@@ -876,14 +806,7 @@ k_bucket_scatter(const PT *__restrict__ pos, const void *__restrict__ mass, int 
     if ((int)hdr[HDR_MODE] != bp.mode) return;
     extern __shared__ __align__(128) unsigned char s_raw[];
     unsigned *s_cur = reinterpret_cast<unsigned *>(s_raw);
-    PT *sring = reinterpret_cast<PT *>(s_raw + (((size_t)bp.W * sizeof(unsigned) + 127) & ~(size_t)127));
-    __shared__ uint64_t bars[8];
-    if (STAGED && threadIdx.x == 0) {
-        for (int i = 0; i < 8; i++) mbar_init(&bars[i], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
     const bool aligned = (reinterpret_cast<uintptr_t>(pos) & 15) == 0;
-    unsigned seq = 0;
     for (int c = blockIdx.x; c < bp.nchunks; c += gridDim.x) {
         const int64_t b = (int64_t)c * bp.chunk;
         const int64_t e = (b + bp.chunk < n) ? b + bp.chunk : n;
@@ -894,7 +817,7 @@ k_bucket_scatter(const PT *__restrict__ pos, const void *__restrict__ mass, int 
         const int wn = min(bp.W, tg.ntiles - lo);
         for (int i = threadIdx.x; i < wn; i += blockDim.x) s_cur[i] = offsets[lo + i] + row[i];
         __syncthreads();
-        chunk_rounds<PT, STAGED>(cpos, cn, sring, bars, bp.nst, seq, aligned, [&](int j0, int nv, const PT (&x)[4][3]) {
+        chunk_rounds<PT>(cpos, cn, aligned, [&](int j0, int nv, const PT (&x)[4][3]) {
             unsigned r[4][3];
             int t[4], k[4];
             bool anyout = false;
@@ -1012,11 +935,7 @@ template <> struct WinD<4> { static constexpr double DMIN = 1.0;
         for (int r = 0; r < 4; r++) w[r] = pcs_kernel(d - (double)r);
     } };
 
-__device__ __forceinline__ unsigned ld_acquire(const unsigned *p) {
-    unsigned v;
-    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
+__device__ __forceinline__ unsigned smem_u32(const void *p) { return (unsigned)__cvta_generic_to_shared(p); }
 // polling load: gpu-scope relaxed (no L1 invalidation per iteration, unlike ld.acquire = LDG.STRONG + CCTL.IVALL);
 // the acquire is one fence after the loop
 __device__ __forceinline__ unsigned ld_relaxed(const unsigned *p) {
@@ -1085,22 +1004,19 @@ template <int SUP, typename MT, typename FT, bool SHIFTED, int FLUSH>
 __global__ void __launch_bounds__(256, FLUSH == 0 ? 4 : 1)
 k_tile_paint(const unsigned *__restrict__ recs, const MT *__restrict__ smass, TileGeom tg,
              const unsigned *__restrict__ offsets, unsigned *__restrict__ hdr, unsigned *__restrict__ flags,
-             unsigned epoch, int knobs, FT *__restrict__ mesh, unsigned *__restrict__ d_off, FT *__restrict__ d_val,
-             unsigned d_cap) {
+             unsigned epoch, FT *__restrict__ mesh, unsigned *__restrict__ d_off, FT *__restrict__ d_val, unsigned d_cap) {
     extern __shared__ __align__(16) unsigned s_all[];
-    const int spread = knobs & 1;                  // diagnosis knobs: bit 0 = spread lanes, bit 1 = acquire-load polling
-    const bool poll_relaxed = !(knobs & 2);
     constexpr int R = TILE + SUP - 1 + (SHIFTED ? 1 : 0);   // == tg.R
     // row pitch in cells: the TMA write-back needs rows that start 16-byte aligned, the ordered one 8-byte cell pairs
     constexpr int RP = FLUSH == 0 ? ((R + 1) & ~1) : ((R + 3) & ~3);
     // x-plane pitch.  CIC, ordered write-back: padded so that the 8 corners of a stencil fall into 8 different banks
-    // (offsets {0, 1, RP, RP+1} + {0, PS}: PS = 8 mod 32 with RP = 18), see the rotated deposit order in accumulate()
+    // (offsets {0, 1, RP, RP+1} + {0, PS}: PS = 8 mod 32 with RP = 18); the padding measurably changes the speed
     constexpr int PS = tile_plane_pitch(SUP, FLUSH, R, RP);
     constexpr int NC = R * PS;
     constexpr int BUFW = (2 * NC + 3) & ~3;                  // words of the accumulator (lo | hi limbs)
     constexpr int H = R - TILE;   // cells with a local coordinate < H are also written by the preceding tile
     constexpr int CAP = R * R * R - TILE * TILE * TILE;      // halo cells = what an interior tile adds
-    constexpr int NT = 256, NW = NT >> 5;
+    constexpr int NT = 256;
     constexpr int HK = (CAP + NT - 1) / NT;                  // halo cells per thread
     unsigned *s_lo = s_all, *s_hi = s_all + NC;
     FT *s_sval = reinterpret_cast<FT *>(s_all + BUFW);                    // stash: value ...
@@ -1120,20 +1036,7 @@ k_tile_paint(const unsigned *__restrict__ recs, const MT *__restrict__ smass, Ti
     if (threadIdx.x == 0) { s_nst[0] = 0; s_nst[1] = 0; }
     const bool small_mesh = (int64_t)tg.gm.x_n * tg.gm.n[1] * tg.gm.n[2] < (1ll << 32);   // 32-bit stash offsets
     const unsigned lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-
-    // Lane-rotated corner order (CIC, ordered write-back): this lane deposits corner j ^ rot at step j.  The neighbouring
-    // records of a spatially coherent catalogue share their stencil cells, and in the same order all their lanes would hit
-    // the same word in every ATOMS; rotated, eight neighbours hit the eight corners, which the padded plane pitch keeps in
-    // eight different banks.  The rotation lives in three signed byte strides and the byte address of the lane's first
-    // corner (four lane constants); the weights of an axis are exchanged where its stride is negative.
-#ifndef NBK_PAINT_ROT
-#define NBK_PAINT_ROT 0      // lane bits that rotate the corner order (x = 4, y = 2, z = 1); 0: fixed order (the rotation removes a
-                             // third of the shared-memory wavefronts, but the pass is issue-bound)
-#endif
-    constexpr bool ROT = (SUP == 2 && FLUSH == 0 && NBK_PAINT_ROT != 0);
-    const unsigned rot = ROT ? (lane & (unsigned)NBK_PAINT_ROT) : 0u;
-    const int sX = (rot & 4u) ? -4 * PS : 4 * PS, sY = (rot & 2u) ? -4 * RP : 4 * RP, sZ = (rot & 1u) ? -4 : 4;
-    const unsigned sbase = smem_u32(s_lo) + ((rot & 4u) ? 4u * PS : 0u) + ((rot & 2u) ? 4u * RP : 0u) + ((rot & 1u) ? 4u : 0u);
+    const unsigned sbase = smem_u32(s_lo);
     constexpr unsigned HIOFF = 4u * (unsigned)NC;          // low limb -> high limb, bytes
     // non-negative deposit q <= 2^31 at the low limb `addr` (shared-window byte address); the carry goes to the high limb
     auto deposit = [&](unsigned addr, unsigned q) {
@@ -1150,28 +1053,23 @@ k_tile_paint(const unsigned *__restrict__ recs, const MT *__restrict__ smass, Ti
     // deposits of the records [b, e) of one bucket into the accumulator (HM: the catalogue carries masses)
     auto accumulate_t = [&](unsigned b, unsigned e, auto hm_tag) {
         constexpr bool HM = decltype(hm_tag)::value;
-        // Particle -> thread map.  spread == 0: thread p takes records p, p + NT, ... (coalesced).  spread != 0: the
-        // lanes of a warp walk 32 separate segments of the bucket (diagnosis knob).
+        // thread p takes records p, p + NT, ... (coalesced)
         const unsigned cnt = e - b;
-        const unsigned seg = (cnt + 31) / 32;               // records per lane segment (spread mode)
-        unsigned idx = spread ? wid : threadIdx.x;          // spread: position within the lane's segment
-        const unsigned step = spread ? (unsigned)NW : (unsigned)NT;
-        const unsigned lim = spread ? min(seg, cnt > lane * seg ? cnt - lane * seg : 0u) : cnt;
-        const unsigned base = spread ? b + lane * seg : b;
+        unsigned idx = threadIdx.x;
         unsigned rn[3] = {0, 0, 0};
         MT mn = (MT)1;
-        if (idx < lim) {
-            const unsigned *rp = recs + 3 * (size_t)(base + idx);
+        if (idx < cnt) {
+            const unsigned *rp = recs + 3 * (size_t)(b + idx);
             rn[0] = rp[0]; rn[1] = rp[1]; rn[2] = rp[2];
-            if (HM) mn = smass[base + idx];
+            if (HM) mn = smass[b + idx];
         }
-        for (; idx < lim; idx += step) {
+        for (; idx < cnt; idx += NT) {
             const unsigned r0 = rn[0], r1 = rn[1], r2 = rn[2];
             const MT mcur = mn;
-            if (idx + step < lim) {                          // next round's record is requested before the deposits
-                const unsigned *rp = recs + 3 * (size_t)(base + idx + step);
+            if (idx + NT < cnt) {                            // next round's record is requested before the deposits
+                const unsigned *rp = recs + 3 * (size_t)(b + idx + NT);
                 rn[0] = rp[0]; rn[1] = rp[1]; rn[2] = rp[2];
-                if (HM) mn = smass[base + idx + step];
+                if (HM) mn = smass[b + idx + NT];
             }
             unsigned u[3] = {r0 << 4, r1 << 4, r2 << 4};
             int l[3] = {(int)(r0 >> 28), (int)(r1 >> 28), (int)(r2 >> 28)};
@@ -1187,15 +1085,6 @@ k_tile_paint(const unsigned *__restrict__ recs, const MT *__restrict__ smass, Ti
                 double fr = (__hiloint2double(0x43300000, (int)u[d]) - 4503599627370496.0) * 2.3283064365386963e-10;
                 WinD<SUP>::eval(WinD<SUP>::DMIN != 0.0 ? WinD<SUP>::DMIN + fr : fr, w[d]);
             }
-            if (ROT) {
-#pragma unroll
-                for (int d = 0; d < 3; d++) {
-                    const bool sw = (rot >> (2 - d)) & 1u;
-                    const double w0 = w[d][0], w1 = w[d][SUP - 1];
-                    w[d][0] = sw ? w1 : w0;
-                    w[d][SUP - 1] = sw ? w0 : w1;
-                }
-            }
             const unsigned a0 = sbase + 4u * (unsigned)(l[0] * PS + l[1] * RP + l[2]);
             const double m = HM ? (double)mcur : 1.0;
             const double mS = m * S;
@@ -1209,26 +1098,23 @@ k_tile_paint(const unsigned *__restrict__ recs, const MT *__restrict__ smass, Ti
 #pragma unroll
                     for (int ry = 0; ry < SUP; ry++) {
                         const double wxy = w[0][rx] * w[1][ry];
-                        const unsigned axy = ROT ? a0 + (unsigned)(rx * sX + ry * sY) : a0 + 4u * (unsigned)(rx * PS + ry * RP);
+                        const unsigned axy = a0 + 4u * (unsigned)(rx * PS + ry * RP);
 #pragma unroll
                         for (int rz = 0; rz < SUP; rz++) {
                             const unsigned q = (unsigned)__double2loint(__fma_rn(wxy, wz[rz], 4503599627370496.0));
-                            deposit(ROT ? axy + (unsigned)(rz * sZ) : axy + 4u * (unsigned)rz, q);
+                            deposit(axy + 4u * (unsigned)rz, q);
                         }
                     }
             } else {
-                const int base0 = l[0] * PS + l[1] * RP + l[2];       // negative weights: signed 64-bit deposits, unrotated
+                const int base0 = l[0] * PS + l[1] * RP + l[2];       // negative weights: signed 64-bit deposits
 #pragma unroll
                 for (int rx = 0; rx < SUP; rx++)
 #pragma unroll
                     for (int ry = 0; ry < SUP; ry++) {
-                        const int jx = (ROT && (rot & 4u)) ? SUP - 1 - rx : rx, jy = (ROT && (rot & 2u)) ? SUP - 1 - ry : ry;
                         const double wxy = w[0][rx] * w[1][ry];
 #pragma unroll
-                        for (int rz = 0; rz < SUP; rz++) {
-                            const int jz = (ROT && (rot & 1u)) ? SUP - 1 - rz : rz;
-                            fixed_add(s_lo, s_hi, base0 + jx * PS + jy * RP + jz, __double2ll_rn(wxy * wz[rz]));
-                        }
+                        for (int rz = 0; rz < SUP; rz++)
+                            fixed_add(s_lo, s_hi, base0 + rx * PS + ry * RP + rz, __double2ll_rn(wxy * wz[rz]));
                     }
             }
         }
@@ -1319,12 +1205,11 @@ k_tile_paint(const unsigned *__restrict__ recs, const MT *__restrict__ smass, Ti
             }
             if (valid) {
                 const unsigned *f = &flags[(nb[0] * tg.nt[1] + nb[1]) * tg.nt[2] + nb[2]];
-                if (poll_relaxed) { while (ld_relaxed(f) < epoch) __nanosleep(32); }
-                else { while (ld_acquire(f) < epoch) __nanosleep(32); }
+                while (ld_relaxed(f) < epoch) __nanosleep(32);
             }
         }
         __syncwarp();
-        if (poll_relaxed) fence_acq_rel_gpu();
+        fence_acq_rel_gpu();
     };
     // one look at the same flags, no waiting (warp-uniform result)
     auto earlier_ready = [&](const TileBox &bx) -> bool {
@@ -1379,7 +1264,7 @@ k_tile_paint(const unsigned *__restrict__ recs, const MT *__restrict__ smass, Ti
             const bool ready = earlier_ready(pbox);
             bool defer = false;
             unsigned dbase = 0;
-            if (!ready && d_cap) {
+            if (!ready) {
                 unsigned tot = 0;
                 for (unsigned i0 = wid * 32; i0 < n; i0 += NT) tot += min(32u, n - i0);
                 if (lane == 0 && tot) dbase = atomicAdd(&hdr[HDR_DEFER], tot);
@@ -1583,7 +1468,7 @@ static void plan_chunks(BucketPlan &p, int64_t n, int maxchunks) {
     if (p.nchunks < 1) p.nchunks = 1;
 }
 
-static void make_plans(int64_t n, const int *nt, int ntiles, size_t pos_size, bool aligned, BucketPlan &coh, BucketPlan &sca,
+static void make_plans(int64_t n, const int *nt, int ntiles, BucketPlan &coh, BucketPlan &sca,
                        int &threads_coh, size_t &smem_coh, int &threads_sca, size_t &smem_sca) {
     auto align128 = [](size_t x) { return (x + 127) & ~(size_t)127; };
     // coherent input: a chunk spans a couple of planes of tiles (+- the displacement blur): 4 planes, at least 4096
@@ -1595,14 +1480,8 @@ static void make_plans(int64_t n, const int *nt, int ntiles, size_t pos_size, bo
     w = env_int("NBK_PAINT_W", (int)w);
     coh.W = ntiles < w ? ntiles : (int)w;
     plan_chunks(coh, n, NBK_CHUNKS_COHERENT);        // refined by the caller once the occupancy is known
-    threads_coh = env_int("NBK_PAINT_THREADS", 512);
-    if (threads_coh > 512 || threads_coh < 64 || threads_coh % 32) threads_coh = 512;     // the coherent kernels are built for <= 512 threads
-    coh.nst = env_int("NBK_PAINT_NST", 2);
-    if (coh.nst < 2) coh.nst = 2;
-    if (coh.nst > 8) coh.nst = 8;
-    size_t ring = (size_t)coh.nst * 4 * threads_coh * 3 * pos_size;
-    coh.staged = (aligned && env_int("NBK_PAINT_STAGED", 0) && align128((size_t)coh.W * 4) + ring <= 224 * 1024) ? 1 : 0;
-    smem_coh = align128((size_t)coh.W * 4) + (coh.staged ? ring : 0);
+    threads_coh = 512;                               // the size the coherent kernels are built for
+    smem_coh = align128((size_t)coh.W * 4);
     coh.wstage = (env_int("NBK_PAINT_WSTAGE", 1) && n < 1400000000ll) ? 1 : 0;   // per-warp record transposition (2 KB per warp; 32-bit word offsets)
     coh.stage_off = (int)smem_coh;
     if (coh.wstage) smem_coh += (size_t)(threads_coh / 32) * 2048;
@@ -1612,10 +1491,7 @@ static void make_plans(int64_t n, const int *nt, int ntiles, size_t pos_size, bo
     sca.W = ntiles < NBK_BLK_SMEM / 4 ? ntiles : NBK_BLK_SMEM / 4;
     plan_chunks(sca, n, NBK_CHUNKS_SCATTERED);
     threads_sca = 1024;
-    sca.nst = 2;
-    ring = (size_t)sca.nst * 4 * threads_sca * 3 * pos_size;
-    sca.staged = (aligned && env_int("NBK_PAINT_STAGED", 0) && align128((size_t)sca.W * 4) + ring <= 224 * 1024) ? 1 : 0;
-    smem_sca = align128((size_t)sca.W * 4) + (sca.staged ? ring : 0);
+    smem_sca = align128((size_t)sca.W * 4);
 }
 
 // capacity of the deferred-add list: a quarter of the tiles may park a full CIC halo (anything beyond waits instead)
@@ -1666,8 +1542,7 @@ static int run_tiled(const void *pos, const void *mass, int64_t n, const PaintGe
     BucketPlan coh, sca;
     int th_c, th_s;
     size_t sm_c, sm_s;
-    const bool aligned = (reinterpret_cast<uintptr_t>(pos) & 15) == 0;
-    make_plans(n, tg.nt, tg.ntiles, sizeof(PT), aligned, coh, sca, th_c, sm_c, th_s, sm_s);
+    make_plans(n, tg.nt, tg.ntiles, coh, sca, th_c, sm_c, th_s, sm_s);
     unsigned *blk = (unsigned *)w;
     {
         size_t a = (size_t)coh.W * NBK_CHUNKS_COHERENT, b = (size_t)sca.W * NBK_CHUNKS_SCATTERED;
@@ -1676,8 +1551,8 @@ static int run_tiled(const void *pos, const void *mass, int64_t n, const PaintGe
     unsigned *recs = (unsigned *)w; w += align256((size_t)n * 12);
     MT *smass = mass ? (MT *)w : nullptr;
     if (mass) w += align256((size_t)n * sizeof(MT));
-    // NBK_PAINT_DEFER=0: wait for unpublished neighbours instead of deferring; NBK_PAINT_DEFER_CAP: smaller list (tests the overflow path)
-    unsigned d_cap = env_int("NBK_PAINT_DEFER", 1) ? (unsigned)nbk_defer_cap(tg.ntiles) : 0u;
+    // NBK_PAINT_DEFER_CAP: smaller list (tests the overflow path)
+    unsigned d_cap = (unsigned)nbk_defer_cap(tg.ntiles);
     {
         const int c = env_int("NBK_PAINT_DEFER_CAP", 0);
         if (c > 0 && (unsigned)c < d_cap) d_cap = (unsigned)c;
@@ -1687,7 +1562,7 @@ static int run_tiled(const void *pos, const void *mass, int64_t n, const PaintGe
     const int mass_f4 = sizeof(MT) == 4;
     int force_mode;
     {
-        const char *e = getenv("NBK_PAINT_BUCKET");      // "coherent" / "scattered" force a configuration (diagnosis)
+        const char *e = getenv("NBK_PAINT_BUCKET");      // "coherent" / "scattered" force the configuration the probe picks
         force_mode = (e && e[0] == 'c') ? 1 : (e && e[0] == 's') ? 0 : -1;
     }
     NBK_CUDA(cudaMemsetAsync(work, 0, 256 + 2 * tb, s));   // header, cnt_w, cnt_o
@@ -1702,17 +1577,10 @@ static int run_tiled(const void *pos, const void *mass, int64_t n, const PaintGe
     // the scatter pass needs more registers), else the last partial wave runs at a fraction of the machine.
     int occ_c = 1, occ_s = 1;
     const size_t sm_cnt = coh.wstage ? (size_t)coh.stage_off : sm_c;      // the count pass does not need the record staging
-    if (coh.staged) {
-        NBK_CUDA(cudaFuncSetAttribute(k_bucket_count<SUP, PT, true, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_c));
-        NBK_CUDA(cudaFuncSetAttribute(k_bucket_scatter<SUP, PT, true, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_c));
-        NBK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_c, k_bucket_count<SUP, PT, true, 512>, th_c, sm_cnt));
-        NBK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_s, k_bucket_scatter<SUP, PT, true, 512>, th_c, sm_c));
-    } else {
-        NBK_CUDA(cudaFuncSetAttribute(k_bucket_count<SUP, PT, false, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_c));
-        NBK_CUDA(cudaFuncSetAttribute(k_bucket_scatter<SUP, PT, false, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_c));
-        NBK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_c, k_bucket_count<SUP, PT, false, 512>, th_c, sm_cnt));
-        NBK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_s, k_bucket_scatter<SUP, PT, false, 512>, th_c, sm_c));
-    }
+    NBK_CUDA(cudaFuncSetAttribute(k_bucket_count<SUP, PT, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_c));
+    NBK_CUDA(cudaFuncSetAttribute(k_bucket_scatter<SUP, PT, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_c));
+    NBK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_c, k_bucket_count<SUP, PT, 512>, th_c, sm_cnt));
+    NBK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_s, k_bucket_scatter<SUP, PT, 512>, th_c, sm_c));
     if (occ_c < 1) occ_c = 1;
     if (occ_s < 1) occ_s = 1;
     if (occ_c > 4) occ_c = 4;
@@ -1728,21 +1596,11 @@ static int run_tiled(const void *pos, const void *mass, int64_t n, const PaintGe
     const int grid_s = sca.nchunks < NBK_SM_COUNT ? sca.nchunks : NBK_SM_COUNT;
 #define LAUNCH_BUCKET(KERN, GRIDC, SMC, ...)                                                                                      \
     do {                                                                                                              \
-        if (coh.staged) {                                                                                             \
-            NBK_CUDA(cudaFuncSetAttribute(KERN<SUP, PT, true, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(SMC))); \
-            KERN<SUP, PT, true, 512><<<GRIDC, th_c, SMC, s>>>(__VA_ARGS__, coh);                                     \
-        } else {                                                                                                      \
-            NBK_CUDA(cudaFuncSetAttribute(KERN<SUP, PT, false, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(SMC))); \
-            KERN<SUP, PT, false, 512><<<GRIDC, th_c, SMC, s>>>(__VA_ARGS__, coh);                                    \
-        }                                                                                                             \
+        NBK_CUDA(cudaFuncSetAttribute(KERN<SUP, PT, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(SMC)));  \
+        KERN<SUP, PT, 512><<<GRIDC, th_c, SMC, s>>>(__VA_ARGS__, coh);                                                \
         NBK_LAUNCHED();                                                                                               \
-        if (sca.staged) {                                                                                             \
-            NBK_CUDA(cudaFuncSetAttribute(KERN<SUP, PT, true, 1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_s)); \
-            KERN<SUP, PT, true, 1024><<<grid_s, th_s, sm_s, s>>>(__VA_ARGS__, sca);                                   \
-        } else {                                                                                                      \
-            NBK_CUDA(cudaFuncSetAttribute(KERN<SUP, PT, false, 1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_s)); \
-            KERN<SUP, PT, false, 1024><<<grid_s, th_s, sm_s, s>>>(__VA_ARGS__, sca);                                  \
-        }                                                                                                             \
+        NBK_CUDA(cudaFuncSetAttribute(KERN<SUP, PT, 1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_s));  \
+        KERN<SUP, PT, 1024><<<grid_s, th_s, sm_s, s>>>(__VA_ARGS__, sca);                                             \
         NBK_LAUNCHED();                                                                                               \
     } while (0)
     // (the plan is the LAST kernel argument of both passes so that one macro serves them)
@@ -1757,13 +1615,6 @@ static int run_tiled(const void *pos, const void *mass, int64_t n, const PaintGe
     LAUNCH_BUCKET(k_bucket_scatter, grid_cs, sm_c, (const PT *)pos, mass, mass_f4, n, tg, ft, hdr, offsets, cnt_w, cur_o, blk, win_lo, recs,
                   (void *)smass);
 #undef LAUNCH_BUCKET
-    int spread_mode;
-    {
-        const char *e = getenv("NBK_PAINT_SPREAD");      // "1": the lanes of a warp walk separate segments of a bucket (diagnosis)
-        spread_mode = (e && e[0] == '1') ? 1 : 0;
-        e = getenv("NBK_PAINT_POLL");                    // "acquire": ld.acquire in the flag poll loop (round-2 baseline)
-        if (e && e[0] == 'a') spread_mode |= 2;
-    }
     // the region edge depends on the mesh being painted (one more cell for the half-cell shifted one); tile ids do not
 #define LAUNCH_TP(SH, FL, MESHP, EPOCH)                                                                                \
     do {                                                                                                              \
@@ -1778,10 +1629,9 @@ static int run_tiled(const void *pos, const void *mass, int64_t n, const PaintGe
         int grid = NBK_SM_COUNT * per_sm;                                                                             \
         if (grid > tg.ntiles) grid = tg.ntiles;                                                                       \
         k_tile_paint<SUP, MT, FT, SH, FL><<<grid, 256, smem, s>>>(recs, smass, tg, offsets, hdr, flags, EPOCH,         \
-                                                                  spread_mode, (FT *)(MESHP), d_off, d_val,           \
-                                                                  (FL) == 0 ? d_cap : 0u);                            \
+                                                                  (FT *)(MESHP), d_off, d_val, d_cap);                \
         NBK_LAUNCHED();                                                                                               \
-        if ((FL) == 0 && d_cap) {                                                                                     \
+        if ((FL) == 0) {                                                                                              \
             k_apply_deferred<FT><<<NBK_SM_COUNT * 4, 256, 0, s>>>(hdr, d_off, d_val, d_cap, (FT *)(MESHP));           \
             NBK_LAUNCHED();                                                                                           \
         }                                                                                                             \

@@ -116,22 +116,8 @@ def _copy_streams(device):
 
 
 def _push_chunks(x_n):
-    """parts the slab exchange of r2c is pipelined in (NBK_FFT_PUSH_CHUNKS, default 4; 1 = y pass, then all copies)"""
-    import os
-    try:
-        n = int(os.environ.get("NBK_FFT_PUSH_CHUNKS", "4"))
-    except ValueError:
-        n = 4
-    return max(1, min(n, int(x_n)))
-
-
-def _transpose_mode():
-    """how the slab transpose of a distributed FFT crosses NVLink: 'push' (line pass into send blocks + one strided bulk
-    copy per peer, default) or 'stores' (the line pass stores every 128..256-byte run straight into the peer's field);
-    NBK_FFT_TRANSPOSE_MODE selects"""
-    import os
-    m = os.environ.get("NBK_FFT_TRANSPOSE_MODE", "push")
-    return m if m in ("push", "stores") else "push"
+    """parts the slab exchange of r2c is pipelined in: 4, or one per x plane when the slab has fewer"""
+    return max(1, min(4, int(x_n)))
 
 
 class SlabLayout(object):
@@ -899,53 +885,37 @@ class RealField(Field):
             work = torch.empty((pm.x_n, Ny, Nzc), dtype=out.value.dtype, device=out.value.device)
             st = pm._peer_stage()
             if st is not None:
-                # z pass locally; y pass writes every output row straight into its owner's staging buffer over
-                # NVLink (fused compute + transpose); barriers bracket the remote writes; x pass reads the staging
+                # z pass locally; y pass into P contiguous send blocks, then one strided bulk copy per peer into its
+                # owner's staging buffer over NVLink; barriers bracket the remote writes; x pass reads the staging
                 # buffer and writes the result field
                 view, ptrs, hdl = st
                 from .._lib import lib as _L
                 with stage("fft_z"):
                     check(_L().nbk_fft_z_forward(_ptr(self.value), _ptr(work), code, pm.x_n * Ny, Nz, _stream()), "fft_z_forward")
-                if _transpose_mode() == "push":
-                    # y pass into P contiguous send blocks, then one strided bulk copy per peer over NVLink
-                    send = torch.empty((P, pm.y_n, pm.x_n, Nzc), dtype=out.value.dtype, device=out.value.device)
-                    nchunk = _push_chunks(pm.x_n)
-                    if nchunk <= 1:
-                        with stage("fft_y_pack"):
-                            check(_L().nbk_fft_lines_pack(_ptr(work), _ptr(send), code, Ny, Nzc, pm.x_n, P, 0, 1.0, _stream()),
-                                  "fft_lines_pack")
-                        hdl.barrier(channel=0)
-                        with stage("fft_y_scatter"):
-                            check(_L().nbk_slab_push(_ptr(send), ptrs, code, pm.y_n, pm.x_n, Nzc, pm.x_start, P, pm.comm.rank,
-                                                     _stream()), "slab_push")
-                    else:
-                        # pipelined: the slab is transformed in `nchunk` parts of x planes; part c travels over NVLink on a
-                        # copy stream (two of them, alternating: two copy engines) while part c + 1 is transformed
-                        hdl.barrier(channel=0)          # every rank is past its previous x pass: the staging buffers are free
-                        main = torch.cuda.current_stream()
-                        copies = _copy_streams(out.value.device)
-                        per = (pm.x_n + nchunk - 1) // nchunk
-                        with stage("fft_y_scatter"):    # (the y pass of all parts + the exposed tail of the copies)
-                            for c in range(nchunk):
-                                o0 = c * per
-                                oc = min(per, pm.x_n - o0)
-                                if oc <= 0:
-                                    break
-                                check(_L().nbk_fft_lines_pack_range(_ptr(work), _ptr(send), code, Ny, Nzc, pm.x_n, o0, oc, P, 0, 1.0,
-                                                                    _stream()), "fft_lines_pack_range")
-                                ev = torch.cuda.Event()
-                                ev.record(main)
-                                cs = copies[c % len(copies)]
-                                cs.wait_event(ev)
-                                check(_L().nbk_slab_push_range(_ptr(send), ptrs, code, pm.y_n, pm.x_n, Nzc, pm.x_start, o0, oc, P,
-                                                               pm.comm.rank, ctypes.c_void_p(cs.cuda_stream)), "slab_push_range")
-                            for cs in copies:
-                                main.wait_stream(cs)
-                else:
-                    hdl.barrier(channel=0)
-                    with stage("fft_y_scatter"):
-                        check(_L().nbk_fft_lines_scatter(_ptr(work), ptrs, code, Ny, Nzc, pm.x_n, pm.x_start, P, 0, 1.0,
-                                                         _stream()), "fft_lines_scatter")
+                send = torch.empty((P, pm.y_n, pm.x_n, Nzc), dtype=out.value.dtype, device=out.value.device)
+                nchunk = _push_chunks(pm.x_n)
+                # pipelined: the slab is transformed in `nchunk` parts of x planes; part c travels over NVLink on a
+                # copy stream (two of them, alternating: two copy engines) while part c + 1 is transformed
+                hdl.barrier(channel=0)          # every rank is past its previous x pass: the staging buffers are free
+                main = torch.cuda.current_stream()
+                copies = _copy_streams(out.value.device)
+                per = (pm.x_n + nchunk - 1) // nchunk
+                with stage("fft_y_scatter"):    # (the y pass of all parts + the exposed tail of the copies)
+                    for c in range(nchunk):
+                        o0 = c * per
+                        oc = min(per, pm.x_n - o0)
+                        if oc <= 0:
+                            break
+                        check(_L().nbk_fft_lines_pack_range(_ptr(work), _ptr(send), code, Ny, Nzc, pm.x_n, o0, oc, P, 0, 1.0,
+                                                            _stream()), "fft_lines_pack_range")
+                        ev = torch.cuda.Event()
+                        ev.record(main)
+                        cs = copies[c % len(copies)]
+                        cs.wait_event(ev)
+                        check(_L().nbk_slab_push_range(_ptr(send), ptrs, code, pm.y_n, pm.x_n, Nzc, pm.x_start, o0, oc, P,
+                                                       pm.comm.rank, ctypes.c_void_p(cs.cuda_stream)), "slab_push_range")
+                    for cs in copies:
+                        main.wait_stream(cs)
                 hdl.barrier(channel=1)
                 scale = float(scale) / (float(Nx) * Ny * Nz)
                 with stage("fft_x"):
@@ -1057,24 +1027,18 @@ class ComplexField(BaseComplexField):
             return out
         st = pm._peer_stage() if P > 1 else None
         if st is not None:
-            # inverse x pass scatters rows into the owners' staging buffers over NVLink (the input is only read);
-            # inverse y pass + z c2r then run locally on the staging buffer
+            # inverse x pass into P contiguous send blocks (the input is only read), one strided bulk copy per peer into
+            # the owners' staging buffers over NVLink; inverse y pass + z c2r then run locally on the staging buffer
             view, ptrs, hdl = st
             Nzc = pm.Nzc
-            if _transpose_mode() == "push":
-                send = torch.empty((P, pm.x_n, pm.y_n, Nzc), dtype=self.value.dtype, device=self.value.device)
-                with stage("ifft_x_pack"):
-                    check(lib().nbk_fft_lines_pack(_ptr(self.value), _ptr(send), code, Nx, Nzc, pm.y_n, P, 1, 1.0, _stream()),
-                          "fft_lines_pack(inverse)")
-                hdl.barrier(channel=0)
-                with stage("ifft_x_scatter"):
-                    check(lib().nbk_slab_push(_ptr(send), ptrs, code, pm.x_n, pm.y_n, Nzc, pm.y_start, P, pm.comm.rank,
-                                              _stream()), "slab_push(inverse)")
-            else:
-                hdl.barrier(channel=0)
-                with stage("ifft_x_scatter"):
-                    check(lib().nbk_fft_lines_scatter(_ptr(self.value), ptrs, code, Nx, Nzc, pm.y_n, pm.y_start, P, 1, 1.0,
-                                                      _stream()), "fft_lines_scatter(inverse)")
+            send = torch.empty((P, pm.x_n, pm.y_n, Nzc), dtype=self.value.dtype, device=self.value.device)
+            with stage("ifft_x_pack"):
+                check(lib().nbk_fft_lines_pack_range(_ptr(self.value), _ptr(send), code, Nx, Nzc, pm.y_n, 0, pm.y_n, P, 1, 1.0,
+                                                     _stream()), "fft_lines_pack_range(inverse)")
+            hdl.barrier(channel=0)
+            with stage("ifft_x_scatter"):
+                check(lib().nbk_slab_push_range(_ptr(send), ptrs, code, pm.x_n, pm.y_n, Nzc, pm.y_start, 0, pm.y_n, P,
+                                                pm.comm.rank, _stream()), "slab_push_range(inverse)")
             hdl.barrier(channel=1)
             with stage("ifft_zy"):
                 check(lib().nbk_fft_zy_backward(_ptr(view), _ptr(out.value), code, pm.x_n, Ny, Nz, _stream()), "fft_zy_backward")

@@ -35,15 +35,19 @@ def main():
     cases = [dict(resampler="cic", interlaced=False, dtype="f8", mode="1d", kw={}),
              dict(resampler="tsc", interlaced=True, dtype="f4", mode="2d", kw=dict(Nmu=4, poles=[0, 2])),
              dict(resampler="pcs", interlaced=False, dtype="f8", mode="1d", kw={})]
-    for tmode, c in [(t, c) for t in ("push", "push-unpipelined", "stores") for c in cases]:
-        # bulk peer copies pipelined with the y pass (default) | y pass, then all copies | fine-grained remote stores
-        os.environ["NBK_FFT_TRANSPOSE_MODE"] = "stores" if tmode == "stores" else "push"
-        os.environ["NBK_FFT_PUSH_CHUNKS"] = "1" if tmode == "push-unpipelined" else "4"
+    peer_stage = None
+    for tmode, c in [(t, c) for t in ("push", "nccl") for c in cases]:
+        # bulk peer copies pipelined with the y pass (default) | pack + NCCL all-to-all + unpack (platforms without
+        # symmetric memory)
+        if tmode == "nccl":
+            os.environ["NBK_FFT_TRANSPOSE"] = "nccl"
         cat = ArrayCatalog({"Position": torch.from_numpy(pos_all[mine]).cuda(), "Weight": torch.from_numpy(w_all[mine]).cuda()},
                            comm=comm, BoxSize=L)
         mesh = cat.to_mesh(Nmesh=N, resampler=c["resampler"], interlaced=c["interlaced"], compensated=True, dtype=c["dtype"])
         r = FFTPower(mesh, mode=c["mode"], **c["kw"])
         real = mesh.compute(mode="real")
+        if tmode == "push":
+            peer_stage = getattr(mesh.pm, "_stage", "unused")
         slabs = comm.allgather(real.numpy())
         if rank == 0:
             cat1 = ArrayCatalog({"Position": torch.from_numpy(pos_all).cuda(), "Weight": torch.from_numpy(w_all).cuda()},
@@ -69,8 +73,7 @@ def main():
             print("case %s [transpose=%s]: %s (real field bit-identical to 1 GPU: %s)" % (c, tmode, "OK" if ok else "MISMATCH", bitexact), flush=True)
             if not ok:
                 failures.append(c)
-    os.environ.pop("NBK_FFT_TRANSPOSE_MODE", None)
-    os.environ.pop("NBK_FFT_PUSH_CHUNKS", None)
+    os.environ.pop("NBK_FFT_TRANSPOSE", None)
     # ---- a dense catalogue on a 256^3 mesh: tiled paint on slabs (ghost tiles, ordered write-back), both orders
     from nbodykit_b200.cosmology import NoWiggleEHPower
     from nbodykit_b200.lab import LinearMesh, LogNormalCatalog
@@ -127,8 +130,8 @@ def main():
         if not ok:
             failures.append("FFTRecon")
     if rank == 0:
-        st = getattr(mesh.pm, "_stage", "unused")
-        print("slab transpose path: %s" % ("NVLink peer-memory scatter" if st not in (None, "unused") else "NCCL all-to-all (%s)" % str(st)), flush=True)
+        st = peer_stage
+        print("slab transpose path of the push leg: %s" % ("NVLink peer-memory push" if st not in (None, "unused") else "NCCL all-to-all (%s)" % str(st)), flush=True)
     flag = torch.tensor([len(failures)], device="cuda")
     dist.broadcast(flag, 0)
     dist.barrier()

@@ -306,11 +306,10 @@ def test_paint_tiled_vs_oracle(cuda, resampler, mesh_dtype, pos_dtype, weighted)
 
 @pytest.mark.parametrize("resampler,pos_dtype,weighted", [("cic", "f4", False), ("cic", "f8", True), ("tsc", "f4", True),
                                                           ("pcs", "f4", False), ("nnb", "f8", False)])
-@pytest.mark.parametrize("knobs", [{}, {"NBK_PAINT_WSTAGE": "0"}, {"NBK_PAINT_DEFER": "0"}, {"NBK_PAINT_DEFER_CAP": "700"},
-                                   {"NBK_PAINT_W": "16"}])
+@pytest.mark.parametrize("knobs", [{}, {"NBK_PAINT_WSTAGE": "0"}, {"NBK_PAINT_DEFER_CAP": "700"}, {"NBK_PAINT_W": "16"}])
 def test_paint_tiled_coherent_plan_variants(cuda, monkeypatch, resampler, pos_dtype, weighted, knobs):
     """the coherent bucketing plan (windowed histogram, per-warp record transposition) and the write-back variants of the
-    tile pass (deferred halo list, its overflow -> wait fallback, plain waiting): cell-sorted input, and the same plan forced
+    tile pass (deferred halo list, its overflow -> wait fallback): cell-sorted input, and the same plan forced
     onto unsorted input; NBK_PAINT_W=16 shrinks the tile window below the 48 tiles of this mesh, so most particles take the
     out-of-window (global atomic) route; all must reproduce the oracle"""
     N, L = [64, 48, 64], [128., 96., 128.]                # power-of-two N/L on x and z, not on y: both record paths
@@ -517,48 +516,18 @@ def test_route_kernels_vs_numpy(cuda):
             start += cnt[r]
 
 
-@pytest.mark.parametrize("shape", [(16, 32, 8), (64, 128, 8), (128, 64, 32), (4, 256, 8), (256, 512, 4), (2, 1024, 16)])
-@pytest.mark.parametrize("dtype", ["f8", "f4"])
-def test_fft_scatter_transpose_two_virtual_ranks(cuda, dtype, shape):
-    """nbk_fft_z_forward + nbk_fft_lines_scatter + nbk_fft_lines_oop == r2c, with the slab transpose done by the y
-    pass writing into 'peer' buffers (two virtual ranks on one GPU: the peers are two buffers of this device)"""
-    import ctypes
-    import torch
-    from nbodykit_b200 import _lib
-    (Nx, Ny, Nz), P = shape, 2
-    Nzc = Nz // 2 + 1
-    rng = np.random.RandomState(17)
-    real = rng.standard_normal((Nx, Ny, Nz)).astype(dtype)
-    want = np.fft.rfftn(real.astype("f8")) / real.size
-    cdt = torch.complex64 if dtype == "f4" else torch.complex128
-    code = 4 if dtype == "f4" else 8
-    Lb = _lib.lib()
-    x_n, y_n = Nx // P, Ny // P
-    stage = [torch.zeros((y_n, Nx, Nzc), dtype=cdt, device="cuda") for _ in range(P)]
-    ptrs = (ctypes.c_void_p * P)(*[t.data_ptr() for t in stage])
-    for r in range(P):      # each virtual rank transforms its x slab and scatters rows to the owners of y
-        slab = torch.from_numpy(real[r * x_n:(r + 1) * x_n].copy()).cuda()
-        work = torch.empty((x_n, Ny, Nzc), dtype=cdt, device="cuda")
-        _lib.check(Lb.nbk_fft_z_forward(ctypes.c_void_p(slab.data_ptr()), ctypes.c_void_p(work.data_ptr()), code, x_n * Ny, Nz, None))
-        _lib.check(Lb.nbk_fft_lines_scatter(ctypes.c_void_p(work.data_ptr()), ptrs, code, Ny, Nzc, x_n, r * x_n, P, 0, 1.0, None))
-    torch.cuda.synchronize()
-    tol = 1e-13 if dtype == "f8" else 2e-6
-    for r in range(P):      # x pass out of place on each rank's transposed field
-        out = torch.empty_like(stage[r])
-        _lib.check(Lb.nbk_fft_lines_oop(ctypes.c_void_p(stage[r].data_ptr()), ctypes.c_void_p(out.data_ptr()), code, Nx, Nzc, Nzc,
-                                        y_n, Nx * Nzc, 0, 1.0 / real.size, None))
-        torch.cuda.synchronize()
-        got = out.cpu().numpy()                                  # [y_n][Nx][Nzc]
-        ref = np.transpose(want[:, r * y_n:(r + 1) * y_n, :], (1, 0, 2))
-        assert np.abs(got - ref).max() <= tol * np.sqrt((np.abs(want) ** 2).mean()) * 10
-
-
-@pytest.mark.parametrize("shape,chunks", [((16, 32, 8), 4), ((8, 256, 16), 3), ((256, 64, 4), 5)])
+# chunks = 1 is the whole slab in one part (the c2r exchange).  The line lengths cover every pack kernel: N < 64 (shared
+# memory), N = 64 and 128 (register I/O), N = 256, 512 and 1024 (TMA; f4 with Nz/2+1 = 3 columns takes the misaligned
+# register-I/O fallback)
+@pytest.mark.parametrize("shape,chunks", [((16, 32, 8), 4), ((8, 256, 16), 3), ((256, 64, 4), 5), ((128, 64, 32), 3),
+                                          ((16, 32, 8), 1), ((64, 128, 8), 1), ((128, 64, 32), 1), ((4, 256, 8), 1),
+                                          ((256, 512, 4), 1), ((2, 1024, 16), 1)])
 @pytest.mark.parametrize("dtype", ["f8", "f4"])
 def test_fft_pack_push_range_two_virtual_ranks(cuda, dtype, shape, chunks):
-    """the pipelined slab exchange of the distributed r2c: nbk_fft_lines_pack_range (y pass of a part of the slab into the
+    """the slab exchange of the distributed r2c / c2r: nbk_fft_lines_pack_range (y pass of a part of the slab into the
     send blocks) + nbk_slab_push_range (strided bulk copies of that part into the owners' transposed fields), part by part,
-    must give the transposed field of the one-shot y pass -- two virtual ranks on one GPU, uneven last part included"""
+    must give the transposed field of the one-shot y pass -- two virtual ranks on one GPU (the peers are two buffers of
+    this device), uneven last part included"""
     import ctypes
     import torch
     from nbodykit_b200 import _lib

@@ -235,16 +235,7 @@ def test_fftrecon_and_projected_power_argument_checks():
         ProjectedFFTPower(d, Nmesh=8, axes=(0, 1, 2))
 
 
-def test_push_chunks_knob(monkeypatch):
-    """parts the slab exchange of the distributed r2c is pipelined in: bounded by the planes of the slab, 1 disables it"""
-    from nbodykit_b200.pmesh.pm import _push_chunks, _transpose_mode
-    monkeypatch.delenv("NBK_FFT_PUSH_CHUNKS", raising=False)
+def test_push_chunks_clamp():
+    """parts the slab exchange of the distributed r2c is pipelined in: 4, bounded by the planes of the slab"""
+    from nbodykit_b200.pmesh.pm import _push_chunks
     assert _push_chunks(128) == 4 and _push_chunks(2) == 2 and _push_chunks(1) == 1
-    monkeypatch.setenv("NBK_FFT_PUSH_CHUNKS", "1")
-    assert _push_chunks(128) == 1
-    monkeypatch.setenv("NBK_FFT_PUSH_CHUNKS", "nonsense")
-    assert _push_chunks(128) == 4
-    monkeypatch.setenv("NBK_FFT_TRANSPOSE_MODE", "stores")
-    assert _transpose_mode() == "stores"
-    monkeypatch.setenv("NBK_FFT_TRANSPOSE_MODE", "other")
-    assert _transpose_mode() == "push"

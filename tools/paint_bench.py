@@ -48,20 +48,16 @@ def main():
     del perm
     ref = None
     cases = (("sorted", pos),) if "--only-sorted" in sys.argv else (("sorted", pos), ("permuted", pp))
-    spreads = ("1", "0") if "--spread-both" in sys.argv else (os.environ.get("NBK_PAINT_SPREAD", ""),)
     tag = " ".join("%s=%s" % (k[10:], v) for k, v in sorted(os.environ.items()) if k.startswith("NBK_PAINT_"))
     for label, p in cases:
-        for spread in spreads:
-            if spread:
-                os.environ["NBK_PAINT_SPREAD"] = spread
-            t = timeit(lambda: pm.paint(p, resampler=res, hold=False, out=real, method='tiled'))
-            print("%s %d^3 %s n=%d %-8s spread=%s [%s]: %.3f ms (median %.3f) -> %.3e part/s, %.0f GB/s algorithmic" % (
-                res, Nmesh, dtype, n, label, spread, tag, t[0], t[1], n / t[0] * 1e3, alg / t[0] / 1e6), flush=True)
-            if ref is None:
-                ref = real.value.clone()
-                print("   sum = %.6f (n = %d)" % (real.csum(), n))
-            else:
-                print("   identical to the first mesh:", bool(torch.equal(ref, real.value)))
+        t = timeit(lambda: pm.paint(p, resampler=res, hold=False, out=real, method='tiled'))
+        print("%s %d^3 %s n=%d %-8s [%s]: %.3f ms (median %.3f) -> %.3e part/s, %.0f GB/s algorithmic" % (
+            res, Nmesh, dtype, n, label, tag, t[0], t[1], n / t[0] * 1e3, alg / t[0] / 1e6), flush=True)
+        if ref is None:
+            ref = real.value.clone()
+            print("   sum = %.6f (n = %d)" % (real.csum(), n))
+        else:
+            print("   identical to the first mesh:", bool(torch.equal(ref, real.value)))
     if check:
         t = timeit(lambda: pm.paint(pos, resampler=res, hold=False, out=real, method='direct'), warm=1, rep=2)
         d = (real.value - ref).abs().max().item()
