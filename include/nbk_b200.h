@@ -162,6 +162,13 @@ int nbk_fft_lines_mixed(const void *src, void *dst, int dtype, int64_t n_line, i
                         int64_t n_outer, int64_t outer_stride, int inverse, double scale, void *stream);
 int nbk_fft_z_mixed(const void *in, void *out, int dtype, int64_t rows, int64_t Nz, int inverse, double scale,
                     void *stream);
+/* Bluestein (chirp-z) passes with the arguments and semantics of the mixed-radix pair above, for sides with a prime
+ * factor above 7 (a cyclic convolution of length M >= 2n - 1, M 7-smooth, done by the mixed-radix stages).  They take
+ * any length within the same limits, 7-smooth lengths included: lines 2 .. 4096; Nz even up to 8192, odd up to 4095. */
+int nbk_fft_lines_bluestein(const void *src, void *dst, int dtype, int64_t n_line, int64_t line_stride, int64_t n_inner,
+                            int64_t n_outer, int64_t outer_stride, int inverse, double scale, void *stream);
+int nbk_fft_z_bluestein(const void *in, void *out, int dtype, int64_t rows, int64_t Nz, int inverse, double scale,
+                        void *stream);
 
 /* the three 1-D passes of the slab-decomposed transform, for the multi-GPU path (P > 1):
  *   zy pass : real slab [x_n][Ny][Nz] -> cplx slab [x_n][Ny][Nzc], r2c along z then FFT along y

@@ -48,6 +48,8 @@ SIGNATURES = {
     "nbk_c2r_mixed": ([_vp, _vp, _i, _pi64, _vp, _vp], _i),
     "nbk_fft_lines_mixed": ([_vp, _vp, _i, _i64, _i64, _i64, _i64, _i64, _i, _d, _vp], _i),
     "nbk_fft_z_mixed": ([_vp, _vp, _i, _i64, _i64, _i, _d, _vp], _i),
+    "nbk_fft_lines_bluestein": ([_vp, _vp, _i, _i64, _i64, _i64, _i64, _i64, _i, _d, _vp], _i),
+    "nbk_fft_z_bluestein": ([_vp, _vp, _i, _i64, _i64, _i, _d, _vp], _i),
     "nbk_fft_zy_forward": ([_vp, _vp, _i, _i64, _i64, _i64, _vp], _i),
     "nbk_fft_zy_backward": ([_vp, _vp, _i, _i64, _i64, _i64, _vp], _i),
     "nbk_fft_lines": ([_vp, _i, _i64, _i64, _i64, _i64, _i64, _i, _d, _vp], _i),

@@ -17,7 +17,9 @@
 // Decimation-in-frequency radix-8 butterflies in registers throughout (+ one radix-4 / radix-2 stage for the remainder of
 // log2 N).  Twiddles: f8-accurate table built on the device with sincospi, staged in shared memory.  Sizes: 2^k.
 // Sides that are products of 2, 3, 5 and 7 (Nx, Ny <= 4096; Nz <= 8192 even, <= 4095 odd) go through the separate
-// mixed-radix entry points at the end of this file (k_fft_lines_mixed, k_fft_z_mixed; nbk_r2c_mixed / nbk_c2r_mixed).
+// mixed-radix entry points at the end of this file (k_fft_lines_mixed, k_fft_z_mixed; nbk_r2c_mixed / nbk_c2r_mixed), and
+// axes whose side has a larger prime factor through the Bluestein passes after them (k_fft_lines_bluestein,
+// k_fft_z_bluestein), which reuse the mixed-radix stages for their convolution.
 #include "common.cuh"
 #include <cuda.h>      // CUtensorMap types only: the encoder comes from cudaGetDriverEntryPoint (no -lcuda)
 #include <map>
@@ -1997,19 +1999,22 @@ __device__ __forceinline__ void mr_fft_tile(C *sm, const C *tw, const MixedPlan 
     }
 }
 
-// perm[k] = position of frequency k after mr_fft_tile (mixed-radix digit reversal).  No barrier.
-__device__ __forceinline__ void mr_build_perm(unsigned short *perm, const MixedPlan &plan) {
-    for (int k = threadIdx.x; k < plan.n; k += blockDim.x) {
-        int rem = k, base = plan.n, pos = 0;
-        for (int s = 0; s < plan.nstage; s++) {
-            const int R = mr_radix(plan, s);
-            const int d = rem % R;
-            rem /= R;
-            base /= R;
-            pos += d * base;
-        }
-        perm[k] = (unsigned short)pos;
+// position of frequency k after mr_fft_tile (mixed-radix digit reversal)
+__device__ __forceinline__ int mr_pos(const MixedPlan &plan, int k) {
+    int rem = k, base = plan.n, pos = 0;
+    for (int s = 0; s < plan.nstage; s++) {
+        const int R = mr_radix(plan, s);
+        const int d = rem % R;
+        rem /= R;
+        base /= R;
+        pos += d * base;
     }
+    return pos;
+}
+
+// perm[k] = mr_pos(plan, k).  No barrier.
+__device__ __forceinline__ void mr_build_perm(unsigned short *perm, const MixedPlan &plan) {
+    for (int k = threadIdx.x; k < plan.n; k += blockDim.x) perm[k] = (unsigned short)mr_pos(plan, k);
 }
 
 // strided tile -> shared [N][pitch] with cp.async; columns beyond the valid width are zero-filled with plain stores
@@ -2377,4 +2382,467 @@ extern "C" int nbk_c2r_mixed(const void *cplx, void *real, int dtype, const int6
     rc = nbk_fft_lines_mixed(c, c, dtype, Ny, Nzc, Nzc, Nx, Ny * Nzc, 1, 1.0, stream);
     if (rc) return rc;
     return nbk_fft_z_mixed(c, real, dtype, Nx * Ny, Nz, 1, 1.0, stream);
+}
+
+// =============================================================================================
+// Bluestein path: lines whose length has a prime factor above 7 (pmesh / pfft hand every side to FFTW; a 1380 box at a
+// 5-unit cell gives 276 = 2^2 3 23).  Separate entry points (nbk_fft_lines_bluestein, nbk_fft_z_bluestein) with the
+// argument lists and limits of the mixed-radix pair; ParticleMesh picks them per axis.
+//   identity : nk = (n^2 + k^2 - (k - n)^2) / 2, so with the chirp c[n] = e^{i pi n^2 / N}
+//              X[k] = conj c[k] sum_n (x[n] conj c[n]) c[k - n], a cyclic convolution of length M, the smallest 7-smooth
+//              number >= 2N - 1, which the mixed-radix stages transform.
+//   tile     : B lines of M points in shared memory, [M][pitch] as in k_fft_lines_mixed.  a = x conj c, zero-padded to M;
+//              forward DIF (mr_fft_tile, digit-reversed output); times the filter spectrum FFT(c) / M, tabulated in the
+//              same digit-reversed order; then the transposed network (mr_fft_tile_dit: the DIT stages in reverse order
+//              take digit-reversed input to natural output) gives the forward DFT F in natural order, and the
+//              convolution is y[k] = F[(M - k) mod M].  No digit-reversal table, no second M-point buffer.
+//   inverse  : IDFT(x)[k] = DFT(x)[(N - k) mod N], as in the mixed path.
+//   tables   : per (N, dtype), cached with the twiddles: conj c[n] (phase from n^2 mod 2N in 64-bit integers, sincospi in
+//              f8) and the filter spectrum (a direct f8 sum of N terms per frequency), rounded to f4 only at the end.
+//              W_M sits in shared memory when it fits beside the tile, else it is read through L2 (f8 at M = 8192: the
+//              one-line tile alone is 128 KB); chirp and filter are always read through L2.
+//   limits   : the mixed path's: complex lines of 2 .. 4096 points (M <= 8192), even Nz <= 8192, odd Nz <= 4095.
+// =============================================================================================
+
+// one DIT stage, the transpose of mr_stage (twiddles first, then the radix-R DFT: both matrices are symmetric)
+template <typename T, typename C, int B, int R>
+__device__ __forceinline__ void mr_stage_dit(C *sm, const C *tw, int N, int Ns) {
+    constexpr int pitch = MrPitch<B>::v;
+    const int Q = Ns / R;
+    const int tws = N / Ns;
+    const int work = (N / R) * B;
+    for (int w = threadIdx.x; w < work; w += blockDim.x) {
+        const int b = w % B, t = w / B;
+        const int blk = t / Q, q = t - blk * Q;
+        C *p = sm + (blk * Ns + q) * pitch + b;
+        const int ti = q * tws;
+        C a[R];
+        a[0] = p[0];
+#pragma unroll
+        for (int m = 1; m < R; m++) a[m] = ti ? cmul(p[m * Q * pitch], tw[m * ti]) : p[m * Q * pitch];
+        dft_mixed<T, C, R>(a);
+#pragma unroll
+        for (int j = 0; j < R; j++) p[j * Q * pitch] = a[j];
+    }
+    __syncthreads();
+}
+
+// forward DFT of B lines held in the digit-reversed order mr_fft_tile leaves, into natural order: the stages of
+// mr_fft_tile transposed, last first.  All threads of the CTA call (it ends with a barrier).
+template <typename T, typename C, int B>
+__device__ __forceinline__ void mr_fft_tile_dit(C *sm, const C *tw, const MixedPlan &plan) {
+    int Ns = 1;
+    for (int s = plan.nstage - 1; s >= 0; s--) {
+        const int R = mr_radix(plan, s);
+        Ns *= R;
+        switch (R) {
+            case 8: mr_stage_dit<T, C, B, 8>(sm, tw, plan.n, Ns); break;
+            case 4: mr_stage_dit<T, C, B, 4>(sm, tw, plan.n, Ns); break;
+            case 2: mr_stage_dit<T, C, B, 2>(sm, tw, plan.n, Ns); break;
+            case 3: mr_stage_dit<T, C, B, 3>(sm, tw, plan.n, Ns); break;
+            case 5: mr_stage_dit<T, C, B, 5>(sm, tw, plan.n, Ns); break;
+            default: mr_stage_dit<T, C, B, 7>(sm, tw, plan.n, Ns); break;
+        }
+    }
+}
+
+// N-point forward DFT of B lines by Bluestein's identity, plan = mr_plan(M), tw = W_M^i.  On entry sm[n * pitch + b],
+// n < N, holds the input (published by a barrier); on exit sm[k * pitch + b], k < N, holds the unscaled DFT in
+// natural order.  All threads of the CTA call (it ends with a barrier).
+template <typename T, typename C, int B>
+__device__ __forceinline__ void bs_fft_tile(C *sm, const C *tw, const C *__restrict__ chirp, const C *__restrict__ filt,
+                                            const MixedPlan &plan, int N) {
+    constexpr int pitch = MrPitch<B>::v;
+    const int M = plan.n;
+    for (int w = threadIdx.x; w < M * B; w += blockDim.x) {
+        const int b = w % B, n = w / B;
+        sm[n * pitch + b] = n < N ? cmul(sm[n * pitch + b], chirp[n]) : C{0, 0};
+    }
+    __syncthreads();
+    mr_fft_tile<T, C, B>(sm, tw, plan, 1);
+    for (int w = threadIdx.x; w < M * B; w += blockDim.x) {
+        const int b = w % B, n = w / B;
+        sm[n * pitch + b] = cmul(sm[n * pitch + b], filt[n]);
+    }
+    __syncthreads();
+    mr_fft_tile_dit<T, C, B>(sm, tw, plan);
+    // y[k] = F[(M - k) mod M]: for k > 0 it lies at M - k >= N (M >= 2N - 1), so no write meets another thread's read
+    for (int w = threadIdx.x; w < N * B; w += blockDim.x) {
+        const int b = w % B, k = w / B;
+        sm[k * pitch + b] = cmul(sm[(k ? M - k : 0) * pitch + b], chirp[k]);
+    }
+    __syncthreads();
+}
+
+// stage W_M^i in shared memory after the tile when the launch made room for it; otherwise read it through L2
+template <typename C>
+__device__ __forceinline__ const C *bs_twiddles(C *smtw, const C *tw_g, int M, int tw_shared) {
+    if (!tw_shared) return tw_g;
+    for (int i = threadIdx.x; i < M; i += blockDim.x) smtw[i] = tw_g[i];
+    return smtw;
+}
+
+// strided line pass with the contract of k_fft_lines_mixed: element(outer, n, inner), dst == src in place (a CTA reads
+// its whole tile before it stores any of it), scale folded into the store.  shared: tile [M][pitch] | W_M^i [M]
+template <typename T, int B>
+__global__ void __launch_bounds__(512, 1)
+k_fft_lines_bluestein(const typename C2<T>::type *src, typename C2<T>::type *dst, const typename C2<T>::type *__restrict__ tw_g,
+                      const typename C2<T>::type *__restrict__ chirp, const typename C2<T>::type *__restrict__ filt,
+                      MixedPlan plan, int N, int64_t line_stride, int64_t n_inner, int64_t tiles_inner, int64_t n_tiles,
+                      int64_t outer_stride, int inverse, T scale, int tw_shared) {
+    typedef typename C2<T>::type C;
+    constexpr int pitch = MrPitch<B>::v;
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    C *sm = reinterpret_cast<C *>(smem_raw);
+    const C *tw = bs_twiddles<C>(sm + (size_t)plan.n * pitch, tw_g, plan.n, tw_shared);
+    for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        const int64_t outer = tile / tiles_inner;
+        const int64_t inner0 = (tile - outer * tiles_inner) * B;
+        const int bvalid = (int)((n_inner - inner0) < B ? (n_inner - inner0) : B);
+        const C *ibase = src + outer * outer_stride + inner0;
+        for (int w = threadIdx.x; w < N * B; w += blockDim.x) {
+            const int b = w % B, n = w / B;
+            sm[n * pitch + b] = b < bvalid ? ibase[(int64_t)n * line_stride + b] : C{0, 0};
+        }
+        __syncthreads();             // (the first time through also publishes tw)
+        bs_fft_tile<T, C, B>(sm, tw, chirp, filt, plan, N);
+        C *obase = dst + outer * outer_stride + inner0;
+        for (int w = threadIdx.x; w < N * B; w += blockDim.x) {
+            const int b = w % B, k = w / B;
+            if (b < bvalid) {
+                const C v = sm[((inverse && k) ? N - k : k) * pitch + b];
+                obase[(int64_t)k * line_stride + b] = C{v.x * scale, v.y * scale};
+            }
+        }
+        __syncthreads();             // everyone is done with the tile before the next load overwrites it
+    }
+}
+
+// z pass with the packing of k_fft_z_mixed: real rows [rows][Nz] <-> complex rows [rows][Nz/2+1]; a tile holds B complex
+// lines of L points, one row each (even Nz, L = Nz/2) or two rows each (odd Nz, L = Nz), transformed by Bluestein over
+// plan = mr_plan(M).  twz = W_Nz^i (the Hermitian split of even rows, read through L2).  shared: tile [M][pitch] | W_M^i
+template <typename T, int B>
+__global__ void __launch_bounds__(256)
+k_fft_z_bluestein(const void *in, void *out, const typename C2<T>::type *__restrict__ twz,
+                  const typename C2<T>::type *__restrict__ tw_g, const typename C2<T>::type *__restrict__ chirp,
+                  const typename C2<T>::type *__restrict__ filt, MixedPlan plan, int Nz, int64_t rows, int inverse, T scale,
+                  int tw_shared) {
+    typedef typename C2<T>::type C;
+    constexpr int pitch = MrPitch<B>::v;
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const bool odd = Nz & 1;
+    const int L = odd ? Nz : Nz / 2;
+    const int Nzc = Nz / 2 + 1;
+    const int rpl = odd ? 2 : 1;                   // real rows per complex line
+    C *sm = reinterpret_cast<C *>(smem_raw);
+    const C *tw = bs_twiddles<C>(sm + (size_t)plan.n * pitch, tw_g, plan.n, tw_shared);
+    const int64_t per_tile = (int64_t)B * rpl;
+    const int64_t n_tiles = (rows + per_tile - 1) / per_tile;
+    const T h = (T)0.5 * scale;
+    for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        const int64_t row0 = tile * per_tile;
+        const int nrows = (int)((rows - row0) < per_tile ? (rows - row0) : per_tile);
+        // ---- load (lanes along the contiguous rows)
+        if (!inverse && !odd) {
+            const C *src = reinterpret_cast<const C *>(static_cast<const T *>(in) + row0 * Nz);
+            for (int w = threadIdx.x; w < L * B; w += blockDim.x) {
+                const int b = w / L, n = w - b * L;
+                sm[n * pitch + b] = b < nrows ? src[(int64_t)b * L + n] : C{0, 0};
+            }
+        } else if (!inverse) {
+            const T *src = static_cast<const T *>(in) + row0 * Nz;
+            for (int w = threadIdx.x; w < L * B; w += blockDim.x) {
+                const int b = w / L, n = w - b * L;
+                const T xa = 2 * b < nrows ? src[(int64_t)(2 * b) * Nz + n] : (T)0;
+                const T xb = 2 * b + 1 < nrows ? src[(int64_t)(2 * b + 1) * Nz + n] : (T)0;
+                sm[n * pitch + b] = C{xa, xb};
+            }
+        } else if (!odd) {
+            // Z[k] = E + i O,  E = X[k] + conj X[L-k],  O = conj(W_Nz^k) (X[k] - conj X[L-k]),  k < L
+            const C *src = static_cast<const C *>(in) + row0 * Nzc;
+            for (int w = threadIdx.x; w < L * B; w += blockDim.x) {
+                const int b = w / L, k = w - b * L;
+                C z = C{0, 0};
+                if (b < nrows) {
+                    const C xk = src[(int64_t)b * Nzc + k];
+                    const C xm = cconj(src[(int64_t)b * Nzc + (L - k)]);
+                    const C e = cadd(xk, xm), d = csub(xk, xm);
+                    const C o = cmul(cconj(twz[k]), d);
+                    z = C{e.x - o.y, e.y + o.x};
+                }
+                sm[k * pitch + b] = z;
+            }
+        } else {
+            // both Hermitian rows rebuilt in the tile: Z[k] = X_a[k] + i X_b[k], Z[Nz-k] = conj X_a[k] + i conj X_b[k]
+            const C *src = static_cast<const C *>(in) + row0 * Nzc;
+            for (int w = threadIdx.x; w < Nzc * B; w += blockDim.x) {
+                const int b = w / Nzc, k = w - b * Nzc;
+                C A = 2 * b < nrows ? src[(int64_t)(2 * b) * Nzc + k] : C{0, 0};
+                C Bv = 2 * b + 1 < nrows ? src[(int64_t)(2 * b + 1) * Nzc + k] : C{0, 0};
+                if (k == 0) { A.y = 0; Bv.y = 0; }          // the k = 0 mode of a real row is real
+                sm[k * pitch + b] = C{A.x - Bv.y, A.y + Bv.x};
+                if (k) sm[(L - k) * pitch + b] = C{A.x + Bv.y, Bv.x - A.y};
+            }
+        }
+        __syncthreads();
+        bs_fft_tile<T, C, B>(sm, tw, chirp, filt, plan, L);
+        // ---- store (the tile is in natural order)
+        if (!inverse && !odd) {
+            // X[k] = 1/2 [ (Z[k] + conj Z[L-k]) - i W_Nz^k (Z[k] - conj Z[L-k]) ],  k = 0 .. L  (Z[L] := Z[0])
+            C *dst = static_cast<C *>(out) + row0 * Nzc;
+            for (int w = threadIdx.x; w < Nzc * B; w += blockDim.x) {
+                const int b = w / Nzc, k = w - b * Nzc;
+                if (b < nrows) {
+                    const C zk = sm[(k == L ? 0 : k) * pitch + b];
+                    const C zm = cconj(sm[(k == 0 ? 0 : L - k) * pitch + b]);
+                    const C e = cadd(zk, zm), o = csub(zk, zm);
+                    const C wo = cmul(twz[k], o);
+                    dst[(int64_t)b * Nzc + k] = C{(e.x + wo.y) * h, (e.y - wo.x) * h};
+                }
+            }
+        } else if (!inverse) {
+            // X_a[k] = (Z[k] + conj Z[-k]) / 2,  X_b[k] = -i (Z[k] - conj Z[-k]) / 2
+            C *dst = static_cast<C *>(out) + row0 * Nzc;
+            for (int w = threadIdx.x; w < Nzc * B; w += blockDim.x) {
+                const int b = w / Nzc, k = w - b * Nzc;
+                if (2 * b < nrows) {
+                    const C zk = sm[k * pitch + b];
+                    const C zm = cconj(sm[(k ? L - k : 0) * pitch + b]);
+                    const C e = cadd(zk, zm), d = csub(zk, zm);
+                    dst[(int64_t)(2 * b) * Nzc + k] = C{e.x * h, e.y * h};
+                    if (2 * b + 1 < nrows) dst[(int64_t)(2 * b + 1) * Nzc + k] = C{d.y * h, -d.x * h};
+                }
+            }
+        } else if (!odd) {
+            // x[2n] + i x[2n+1] = sum_k Z[k] e^{+2 pi i k n / L} = DFT(Z)[(L - n) mod L]
+            C *dst = reinterpret_cast<C *>(static_cast<T *>(out) + row0 * Nz);
+            for (int w = threadIdx.x; w < L * B; w += blockDim.x) {
+                const int b = w / L, n = w - b * L;
+                if (b < nrows) {
+                    const C v = sm[(n ? L - n : 0) * pitch + b];
+                    dst[(int64_t)b * L + n] = C{v.x * scale, v.y * scale};
+                }
+            }
+        } else {
+            T *dst = static_cast<T *>(out) + row0 * Nz;
+            for (int w = threadIdx.x; w < L * B; w += blockDim.x) {
+                const int b = w / L, n = w - b * L;
+                if (2 * b < nrows) {
+                    const C v = sm[(n ? L - n : 0) * pitch + b];
+                    dst[(int64_t)(2 * b) * Nz + n] = v.x * scale;
+                    if (2 * b + 1 < nrows) dst[(int64_t)(2 * b + 1) * Nz + n] = v.y * scale;
+                }
+            }
+        }
+        __syncthreads();
+    }
+}
+
+// chirp[n] = conj c[n] = e^{-i pi n^2 / N}; the phase is reduced exactly (n^2 mod 2N) before sincospi
+template <typename T>
+__global__ void k_bs_chirp(typename C2<T>::type *chirp, int N) {
+    const int n = blockIdx.x * blockDim.x + threadIdx.x;
+    if (n < N) {
+        double s, c;
+        sincospi((double)(((int64_t)n * n) % (2 * (int64_t)N)) / (double)N, &s, &c);
+        chirp[n].x = (T)c;
+        chirp[n].y = (T)-s;
+    }
+}
+
+// filt[mr_pos(plan, k)] = FFT(b)[k] / M for the filter b[m] = b[M - m] = c[m] (m < N), zero between.  b is even, so
+// FFT(b)[k] = 1 + 2 sum_{m=1}^{N-1} c[m] cos(2 pi m k / M): one warp per frequency, f8 throughout.
+template <typename T>
+__global__ void k_bs_filter(typename C2<T>::type *filt, int N, MixedPlan plan) {
+    const int M = plan.n;
+    const int lane = threadIdx.x & 31;
+    const int64_t k = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (k >= M) return;                            // (whole warps)
+    double re = 0.0, im = 0.0;
+    for (int m = 1 + lane; m < N; m += 32) {
+        double s, c;
+        sincospi((double)(((int64_t)m * m) % (2 * (int64_t)N)) / (double)N, &s, &c);
+        const double ck = cospi(2.0 * (double)((m * k) % M) / (double)M);
+        re += c * ck;
+        im += s * ck;
+    }
+    for (int o = 16; o; o >>= 1) {
+        re += __shfl_xor_sync(0xffffffffu, re, o);
+        im += __shfl_xor_sync(0xffffffffu, im, o);
+    }
+    if (lane == 0) {
+        typename C2<T>::type v;
+        v.x = (T)((1.0 + 2.0 * re) / M);
+        v.y = (T)(2.0 * im / M);
+        filt[mr_pos(plan, (int)k)] = v;
+    }
+}
+
+// convolution length of an n-point Bluestein transform: the smallest 7-smooth M >= 2n - 1
+static int bs_len(int n) {
+    int m = 2 * n - 1;
+    while (!is_7smooth(m)) m++;
+    return m;
+}
+
+// chirp [N] followed by the filter spectrum [M], one allocation per (device, N, dtype), kept in the twiddle map under
+// the dtype code + NBK_BS_KEY
+#define NBK_BS_KEY 1000
+static int get_bluestein(int N, int dtype, cudaStream_t s, void **chirp, void **filt) {
+    const int M = bs_len(N);
+    const size_t cs = dtype == NBK_F4 ? 8 : 16;
+    int dev = 0;
+    NBK_CUDA(cudaGetDevice(&dev));
+    std::lock_guard<std::mutex> lock(g_tw_mutex);
+    auto key = std::make_tuple(dev, N, dtype + NBK_BS_KEY);
+    auto it = g_tw.find(key);
+    void *p = nullptr;
+    if (it != g_tw.end()) {
+        p = it->second;
+    } else {
+        NBK_CUDA(cudaMalloc(&p, (size_t)(N + M) * cs));
+        void *f = (char *)p + (size_t)N * cs;
+        const MixedPlan plan = mr_plan(M);
+        const int gc = (N + 255) / 256, gf = (M + 7) / 8;     // filter: 8 warps per block
+        if (dtype == NBK_F4) k_bs_chirp<float><<<gc, 256, 0, s>>>((float2 *)p, N);
+        else k_bs_chirp<double><<<gc, 256, 0, s>>>((double2 *)p, N);
+        NBK_LAUNCHED();
+        if (dtype == NBK_F4) k_bs_filter<float><<<gf, 256, 0, s>>>((float2 *)f, N, plan);
+        else k_bs_filter<double><<<gf, 256, 0, s>>>((double2 *)f, N, plan);
+        NBK_LAUNCHED();
+        // the tables must be visible to later launches on other streams as well
+        NBK_CUDA(cudaStreamSynchronize(s));
+        g_tw[key] = p;
+    }
+    *chirp = p;
+    *filt = (char *)p + (size_t)N * cs;
+    return NBK_OK;
+}
+
+// complex line length n: 2 .. 4096, any factors
+static int check_line_bluestein(const char *who, int64_t n) {
+    NBK_CHECK_ARG(n >= 2 && n <= NBK_MR_MAX_LINE,
+                  "%s: line length %lld unsupported: the Bluestein FFT takes lengths 2 .. 4096", who, (long long)n);
+    return NBK_OK;
+}
+
+static int check_z_bluestein(const char *who, int64_t Nz) {
+    NBK_CHECK_ARG(Nz >= 2 && ((Nz % 2 == 0 && Nz <= 2 * NBK_MR_MAX_LINE) || (Nz % 2 && Nz < NBK_MR_MAX_LINE)),
+                  "%s: Nz = %lld unsupported: the Bluestein z pass takes even lengths up to 8192 or odd lengths up to 4095",
+                  who, (long long)Nz);
+    return NBK_OK;
+}
+
+// shared bytes of one M-point tile of B lines, with or without W_M beside it
+template <typename C>
+static size_t bs_smem(int M, int B, bool tw_shared) {
+    return ((size_t)M * (B > 1 ? B + 1 : 1) + (tw_shared ? M : 0)) * sizeof(C) + 16;
+}
+
+template <typename T>
+static int launch_lines_bluestein(const void *src, void *dst, int N, int64_t line_stride, int64_t n_inner, int64_t n_outer,
+                                  int64_t outer_stride, int inverse, double scale, cudaStream_t s) {
+    typedef typename C2<T>::type C;
+    const int dtype = sizeof(T) == 4 ? NBK_F4 : NBK_F8;
+    const int M = bs_len(N);
+    void *tw, *chirp, *filt;
+    int rc = get_twiddle(M, dtype, s, &tw);
+    if (rc) return rc;
+    rc = get_bluestein(N, dtype, s, &chirp, &filt);
+    if (rc) return rc;
+    // 128-byte runs while two CTAs per SM fit, narrower for long lines
+    int B = 128 / (int)sizeof(C);
+    while (B > 1 && (bs_smem<C>(M, B, true) > 110 * 1024 || B / 2 >= n_inner)) B >>= 1;
+    const int tw_shared = bs_smem<C>(M, B, true) <= 227 * 1024;
+    const size_t smem = bs_smem<C>(M, B, tw_shared);
+    NBK_CHECK_ARG(smem <= 227 * 1024, "fft_lines_bluestein: N=%d does not fit in shared memory", N);
+    const int64_t tiles_inner = (n_inner + B - 1) / B;
+    const int64_t n_tiles = tiles_inner * n_outer;
+    int per_sm = (int)((227 * 1024) / (smem + 1024));
+    if (per_sm < 1) per_sm = 1;
+    if (per_sm > 8) per_sm = 8;
+    const int64_t g = n_tiles < (int64_t)NBK_SM_COUNT * per_sm ? n_tiles : (int64_t)NBK_SM_COUNT * per_sm;
+    const int nthreads = (per_sm == 1 && (int64_t)M * B >= 4096) ? 512 : 256;
+    const MixedPlan plan = mr_plan(M);
+#define LAUNCH_LB(BB)                                                                                                  \
+    case BB:                                                                                                           \
+        NBK_CUDA(cudaFuncSetAttribute(k_fft_lines_bluestein<T, BB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+        k_fft_lines_bluestein<T, BB><<<(int)g, nthreads, smem, s>>>((const C *)src, (C *)dst, (const C *)tw, (const C *)chirp, \
+                                                                     (const C *)filt, plan, N, line_stride, n_inner,      \
+                                                                     tiles_inner, n_tiles, outer_stride, inverse, (T)scale, \
+                                                                     tw_shared);                                          \
+        break;
+    switch (B) {
+        LAUNCH_LB(1) LAUNCH_LB(2) LAUNCH_LB(4) LAUNCH_LB(8) LAUNCH_LB(16)
+        default: nbk_set_error("fft_lines_bluestein: internal tile width %d", B); return NBK_ERR_ARG;
+    }
+#undef LAUNCH_LB
+    NBK_LAUNCHED();
+    return NBK_OK;
+}
+
+template <typename T>
+static int launch_z_bluestein(const void *in, void *out, int64_t rows, int Nz, int inverse, double scale, cudaStream_t s) {
+    typedef typename C2<T>::type C;
+    const int dtype = sizeof(T) == 4 ? NBK_F4 : NBK_F8;
+    const bool odd = Nz & 1;
+    const int L = odd ? Nz : Nz / 2;
+    const int M = bs_len(L);
+    void *twz, *tw, *chirp, *filt;
+    int rc = get_twiddle(Nz, dtype, s, &twz);
+    if (rc) return rc;
+    rc = get_twiddle(M, dtype, s, &tw);
+    if (rc) return rc;
+    rc = get_bluestein(L, dtype, s, &chirp, &filt);
+    if (rc) return rc;
+    const int64_t lines = odd ? (rows + 1) / 2 : rows;
+    // B rows per tile: as many as leave two CTAs per SM; long rows take the whole SM
+    int B = 16;
+    while (B > 1 && (bs_smem<C>(M, B, true) > 110 * 1024 || B / 2 >= lines)) B >>= 1;
+    const int tw_shared = bs_smem<C>(M, B, true) <= 227 * 1024;
+    const size_t smem = bs_smem<C>(M, B, tw_shared);
+    NBK_CHECK_ARG(smem <= 227 * 1024, "fft_z_bluestein: Nz=%d does not fit in shared memory", Nz);
+    const int64_t n_tiles = (lines + B - 1) / B;
+    int per_sm = (int)((227 * 1024) / (smem + 1024));
+    if (per_sm < 1) per_sm = 1;
+    if (per_sm > 8) per_sm = 8;
+    const int64_t g = n_tiles < (int64_t)NBK_SM_COUNT * per_sm ? n_tiles : (int64_t)NBK_SM_COUNT * per_sm;
+    const MixedPlan plan = mr_plan(M);
+#define LAUNCH_ZB(BB)                                                                                                  \
+    case BB:                                                                                                           \
+        NBK_CUDA(cudaFuncSetAttribute(k_fft_z_bluestein<T, BB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+        k_fft_z_bluestein<T, BB><<<(int)g, 256, smem, s>>>(in, out, (const C *)twz, (const C *)tw, (const C *)chirp,       \
+                                                            (const C *)filt, plan, Nz, rows, inverse, (T)scale, tw_shared); \
+        break;
+    switch (B) {
+        LAUNCH_ZB(1) LAUNCH_ZB(2) LAUNCH_ZB(4) LAUNCH_ZB(8) LAUNCH_ZB(16)
+        default: nbk_set_error("fft_z_bluestein: internal tile width %d", B); return NBK_ERR_ARG;
+    }
+#undef LAUNCH_ZB
+    NBK_LAUNCHED();
+    return NBK_OK;
+}
+
+extern "C" int nbk_fft_lines_bluestein(const void *src, void *dst, int dtype, int64_t n_line, int64_t line_stride,
+                                       int64_t n_inner, int64_t n_outer, int64_t outer_stride, int inverse, double scale,
+                                       void *stream) {
+    NBK_CHECK_ARG(dtype == NBK_F4 || dtype == NBK_F8, "fft_lines_bluestein: bad dtype %d", dtype);
+    int rc = check_line_bluestein("fft_lines_bluestein", n_line);
+    if (rc) return rc;
+    if (n_inner <= 0 || n_outer <= 0) return NBK_OK;
+    cudaStream_t s = (cudaStream_t)stream;
+    if (dtype == NBK_F4)
+        return launch_lines_bluestein<float>(src, dst, (int)n_line, line_stride, n_inner, n_outer, outer_stride, inverse, scale, s);
+    return launch_lines_bluestein<double>(src, dst, (int)n_line, line_stride, n_inner, n_outer, outer_stride, inverse, scale, s);
+}
+
+extern "C" int nbk_fft_z_bluestein(const void *in, void *out, int dtype, int64_t rows, int64_t Nz, int inverse, double scale,
+                                   void *stream) {
+    NBK_CHECK_ARG(dtype == NBK_F4 || dtype == NBK_F8, "fft_z_bluestein: bad dtype %d", dtype);
+    int rc = check_z_bluestein("fft_z_bluestein", Nz);
+    if (rc) return rc;
+    if (rows <= 0) return NBK_OK;
+    cudaStream_t s = (cudaStream_t)stream;
+    return (dtype == NBK_F4) ? launch_z_bluestein<float>(in, out, rows, (int)Nz, inverse, scale, s)
+                             : launch_z_bluestein<double>(in, out, rows, (int)Nz, inverse, scale, s);
 }

@@ -37,12 +37,53 @@ def _real_typestr(dtype):
     raise TypeError("unsupported mesh dtype %s" % str(dtype))
 
 
+def _smooth7(n):
+    """n is a product of 2, 3, 5 and 7"""
+    if n < 1:
+        return False
+    for p in (2, 3, 5, 7):
+        while n % p == 0:
+            n //= p
+    return n == 1
+
+
 def _stream():
     return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def _ptr(t):
     return ctypes.c_void_p(t.data_ptr() if t is not None else None)
+
+
+def _r2c_one_gpu(pm, real, cplx, scale):
+    """whole-mesh r2c on one GPU of a mesh that is not all powers of two: nbk_r2c_mixed when every side is 7-smooth,
+    else its three passes, z, y and x (with the normalisation), each from pm._z_pass / pm._line_pass"""
+    code = _CODE[pm.typestr]
+    if not any(pm.bluestein):
+        check(lib().nbk_r2c_mixed(_ptr(real), _ptr(cplx), code, pm._nmesh_c, float(scale), _stream()), "nbk_r2c_mixed")
+        return
+    Nx, Ny, Nz = [int(v) for v in pm.Nmesh]
+    Nzc = Nz // 2 + 1
+    check(pm._z_pass()(_ptr(real), _ptr(cplx), code, Nx * Ny, Nz, 0, 1.0, _stream()), "fft_z")
+    check(pm._line_pass(1)(_ptr(cplx), _ptr(cplx), code, Ny, Nzc, Nzc, Nx, Ny * Nzc, 0, 1.0, _stream()), "fft_lines(y)")
+    check(pm._line_pass(0)(_ptr(cplx), _ptr(cplx), code, Nx, Ny * Nzc, Ny * Nzc, 1, 0, 0,
+                           float(scale) / (float(Nx) * Ny * Nz), _stream()), "fft_lines(x)")
+
+
+def _c2r_one_gpu(pm, cplx, real, work):
+    """the mirror of _r2c_one_gpu, unnormalised.  `cplx` is preserved when `work` (its shape) is given, else
+    overwritten"""
+    code = _CODE[pm.typestr]
+    if not any(pm.bluestein):
+        check(lib().nbk_c2r_mixed(_ptr(cplx), _ptr(real), code, pm._nmesh_c, _ptr(work), _stream()), "nbk_c2r_mixed")
+        return
+    Nx, Ny, Nz = [int(v) for v in pm.Nmesh]
+    Nzc = Nz // 2 + 1
+    c = cplx if work is None else work
+    # the x pass reads `cplx` and writes `c` (out of place when work is given)
+    check(pm._line_pass(0)(_ptr(cplx), _ptr(c), code, Nx, Ny * Nzc, Ny * Nzc, 1, 0, 1, 1.0, _stream()), "fft_lines(x)")
+    check(pm._line_pass(1)(_ptr(c), _ptr(c), code, Ny, Nzc, Nzc, Nx, Ny * Nzc, 1, 1.0, _stream()), "fft_lines(y)")
+    check(pm._z_pass()(_ptr(c), _ptr(real), code, Nx * Ny, Nz, 1, 1.0, _stream()), "fft_z")
 
 
 def current_device():
@@ -228,8 +269,10 @@ class ParticleMesh(object):
         self.Nzc = Nz if self.cplx else Nz // 2 + 1      # stored length of the last axis of a ComplexField
         self.transposed = P > 1
         # every side a power of two: the radix-8 kernels (and, with P > 1, the NVLink peer transpose); otherwise the
-        # mixed-radix transform, whose entry points check the sizes it takes (products of 2, 3, 5 and 7)
+        # mixed-radix passes, whose entry points check the sizes they take
         self.pow2 = all(n > 0 and n & (n - 1) == 0 for n in (Nx, Ny, Nz))
+        # of those, the axes (x, y, z) whose side has a prime factor above 7 take the Bluestein passes instead
+        self.bluestein = tuple(not _smooth7(n) for n in (Nx, Ny, Nz))
         self._nmesh_c = iarr(self.Nmesh)
         self._box_c = darr(self.BoxSize)
         self._coords = {}
@@ -257,6 +300,14 @@ class ParticleMesh(object):
         if (Nm == self.Nmesh).all() and numpy.allclose(BoxSize, self.BoxSize) and numpy.dtype(dtype) == numpy.dtype(self.dtype):
             return self
         return ParticleMesh(BoxSize=BoxSize, Nmesh=Nm, dtype=dtype, comm=self.comm)
+
+    # ---- the passes of a mesh that is not all powers of two
+    def _line_pass(self, axis):
+        """complex line pass along axis 0 (x) or 1 (y): Bluestein for a side with a prime factor above 7"""
+        return lib().nbk_fft_lines_bluestein if self.bluestein[axis] else lib().nbk_fft_lines_mixed
+
+    def _z_pass(self):
+        return lib().nbk_fft_z_bluestein if self.bluestein[2] else lib().nbk_fft_z_mixed
 
     def create(self, type=None, base=None, value=None, mode=None):
         type = _typestr_to_type(type if type is not None else mode)
@@ -940,8 +991,9 @@ class RealField(Field):
         return out
 
     def _r2c_mixed(self, out, scale):
-        """r2c for sides that are not all powers of two (mixed-radix kernels).  P > 1: z pass, y lines, pack, NCCL
-        all-to-all, unpack, x lines with the normalisation"""
+        """r2c for sides that are not all powers of two (mixed-radix kernels, Bluestein ones on the axes
+        ParticleMesh.bluestein flags).  P > 1: z pass, y lines, pack, NCCL all-to-all, unpack, x lines with the
+        normalisation"""
         pm = self.pm
         L = lib()
         code = _CODE[pm.typestr]
@@ -950,19 +1002,19 @@ class RealField(Field):
         if pm.cplx:
             half = torch.empty((Nx, Ny, Nz // 2 + 1), dtype=out.value.dtype, device=out.value.device)
             with stage("r2c"):
-                check(L.nbk_r2c_mixed(_ptr(self.value), _ptr(half), code, pm._nmesh_c, float(scale), _stream()), "nbk_r2c_mixed")
+                _r2c_one_gpu(pm, self.value, half, scale)
                 check(L.nbk_hermitian_expand(_ptr(half), _ptr(out.value), code, pm._nmesh_c, _stream()), "nbk_hermitian_expand")
         elif P == 1:
             with stage("r2c"):
-                check(L.nbk_r2c_mixed(_ptr(self.value), _ptr(out.value), code, pm._nmesh_c, float(scale), _stream()), "nbk_r2c_mixed")
+                _r2c_one_gpu(pm, self.value, out.value, scale)
         else:
             Nzc = pm.Nzc
             work = torch.empty((pm.x_n, Ny, Nzc), dtype=out.value.dtype, device=out.value.device)
             send = torch.empty_like(work)
             with stage("fft_zy"):
-                check(L.nbk_fft_z_mixed(_ptr(self.value), _ptr(work), code, pm.x_n * Ny, Nz, 0, 1.0, _stream()), "fft_z_mixed")
-                check(L.nbk_fft_lines_mixed(_ptr(work), _ptr(work), code, Ny, Nzc, Nzc, pm.x_n, Ny * Nzc, 0, 1.0, _stream()),
-                      "fft_lines_mixed(y)")
+                check(pm._z_pass()(_ptr(self.value), _ptr(work), code, pm.x_n * Ny, Nz, 0, 1.0, _stream()), "fft_z")
+                check(pm._line_pass(1)(_ptr(work), _ptr(work), code, Ny, Nzc, Nzc, pm.x_n, Ny * Nzc, 0, 1.0, _stream()),
+                      "fft_lines(y)")
             with stage("fft_pack"):
                 check(L.nbk_transpose_pack(_ptr(work), _ptr(send), code, pm.x_n, Ny, Nzc, P, _stream()), "transpose_pack")
             recv = torch.view_as_real(work).view(-1)
@@ -972,8 +1024,8 @@ class RealField(Field):
                 check(L.nbk_transpose_unpack(_ptr(recv), _ptr(out.value), code, pm.y_n, Nx, Nzc, P, _stream()), "transpose_unpack")
             scale = float(scale) / (float(Nx) * Ny * Nz)
             with stage("fft_x"):
-                check(L.nbk_fft_lines_mixed(_ptr(out.value), _ptr(out.value), code, Nx, Nzc, Nzc, pm.y_n, Nx * Nzc, 0, scale,
-                                            _stream()), "fft_lines_mixed(x)")
+                check(pm._line_pass(0)(_ptr(out.value), _ptr(out.value), code, Nx, Nzc, Nzc, pm.y_n, Nx * Nzc, 0, scale,
+                                       _stream()), "fft_lines(x)")
         out.attrs = dict(self.attrs)
         return out
 
@@ -1062,8 +1114,8 @@ class ComplexField(BaseComplexField):
         return out
 
     def _c2r_mixed(self, out):
-        """c2r for sides that are not all powers of two (mixed-radix kernels), the mirror of RealField._r2c_mixed.
-        The complex buffer is preserved."""
+        """c2r for sides that are not all powers of two (mixed-radix kernels, Bluestein ones on the axes
+        ParticleMesh.bluestein flags), the mirror of RealField._r2c_mixed.  The complex buffer is preserved."""
         pm = self.pm
         L = lib()
         code = _CODE[pm.typestr]
@@ -1073,17 +1125,17 @@ class ComplexField(BaseComplexField):
             half = torch.empty((Nx, Ny, Nz // 2 + 1), dtype=self.value.dtype, device=self.value.device)
             with stage("c2r"):
                 check(L.nbk_hermitian_compress(_ptr(self.value), _ptr(half), code, Nx * Ny, Nz, _stream()), "nbk_hermitian_compress")
-                check(L.nbk_c2r_mixed(_ptr(half), _ptr(out.value), code, pm._nmesh_c, None, _stream()), "nbk_c2r_mixed")
+                _c2r_one_gpu(pm, half, out.value, None)
         elif P == 1:
             work = torch.empty_like(self.value)
             with stage("c2r"):
-                check(L.nbk_c2r_mixed(_ptr(self.value), _ptr(out.value), code, pm._nmesh_c, _ptr(work), _stream()), "nbk_c2r_mixed")
+                _c2r_one_gpu(pm, self.value, out.value, work)
         else:
             Nzc = pm.Nzc
             work = self.value.clone()
             with stage("ifft_x"):
-                check(L.nbk_fft_lines_mixed(_ptr(work), _ptr(work), code, Nx, Nzc, Nzc, pm.y_n, Nx * Nzc, 1, 1.0, _stream()),
-                      "fft_lines_mixed(x)")
+                check(pm._line_pass(0)(_ptr(work), _ptr(work), code, Nx, Nzc, Nzc, pm.y_n, Nx * Nzc, 1, 1.0, _stream()),
+                      "fft_lines(x)")
             send = torch.empty_like(work)
             check(L.nbk_transpose_pack_back(_ptr(work), _ptr(send), code, pm.y_n, Nx, Nzc, P, _stream()), "pack_back")
             recv = torch.view_as_real(work).view(-1)
@@ -1091,9 +1143,9 @@ class ComplexField(BaseComplexField):
             slab = torch.view_as_real(send).view(-1)
             check(L.nbk_transpose_unpack_back(_ptr(recv), _ptr(slab), code, pm.x_n, Ny, Nzc, P, _stream()), "unpack_back")
             with stage("ifft_zy"):
-                check(L.nbk_fft_lines_mixed(_ptr(slab), _ptr(slab), code, Ny, Nzc, Nzc, pm.x_n, Ny * Nzc, 1, 1.0, _stream()),
-                      "fft_lines_mixed(y)")
-                check(L.nbk_fft_z_mixed(_ptr(slab), _ptr(out.value), code, pm.x_n * Ny, Nz, 1, 1.0, _stream()), "fft_z_mixed")
+                check(pm._line_pass(1)(_ptr(slab), _ptr(slab), code, Ny, Nzc, Nzc, pm.x_n, Ny * Nzc, 1, 1.0, _stream()),
+                      "fft_lines(y)")
+                check(pm._z_pass()(_ptr(slab), _ptr(out.value), code, pm.x_n * Ny, Nz, 1, 1.0, _stream()), "fft_z")
         out.attrs = dict(self.attrs)
         return out
 

@@ -6,7 +6,8 @@
 Every case is timed with CUDA events after warm-up (median of --reps calls).  Effective bandwidth counts 6x the real
 field's bytes per transform (three passes, each one read and one write of a field of about that size) and is compared
 with the 3.35 TB/s HBM3 data-sheet figure of the H100 SXM.  For sides that are not powers of two the three passes of
-the mixed-radix r2c (z, y, x) are also timed one by one.  The card's name and power limit are printed with the numbers.
+the r2c (z, y, x) are also timed one by one: the mixed-radix passes, and the Bluestein ones on axes whose side has a
+prime factor above 7.  The card's name and power limit are printed with the numbers.
 """
 import argparse
 import ctypes
@@ -53,18 +54,17 @@ def _time(fn, warmup, reps):
 
 
 def _passes(pm, r, c, warmup, reps):
-    """ms of the z pass, the y lines and the x lines of the mixed-radix r2c"""
+    """ms of the z pass, the y lines and the x lines of the r2c, each the pass ParticleMesh picks for its axis"""
     L = _lib.lib()
     code = 4 if pm.typestr == "f4" else 8
     Nx, Ny, Nz = [int(v) for v in pm.Nmesh]
     Nzc = Nz // 2 + 1
     rp, cp = ctypes.c_void_p(r.value.data_ptr()), ctypes.c_void_p(c.value.data_ptr())
     out = {}
-    out["z"] = _time(lambda: _lib.check(L.nbk_fft_z_mixed(rp, cp, code, Nx * Ny, Nz, 0, 1.0, None)), warmup, reps)
-    out["y"] = _time(lambda: _lib.check(L.nbk_fft_lines_mixed(cp, cp, code, Ny, Nzc, Nzc, Nx, Ny * Nzc, 0, 1.0, None)),
-                     warmup, reps)
-    out["x"] = _time(lambda: _lib.check(L.nbk_fft_lines_mixed(cp, cp, code, Nx, Ny * Nzc, Ny * Nzc, 1, 0, 0, 1.0, None)),
-                     warmup, reps)
+    zp, yp, xp = pm._z_pass(), pm._line_pass(1), pm._line_pass(0)
+    out["z"] = _time(lambda: _lib.check(zp(rp, cp, code, Nx * Ny, Nz, 0, 1.0, None)), warmup, reps)
+    out["y"] = _time(lambda: _lib.check(yp(cp, cp, code, Ny, Nzc, Nzc, Nx, Ny * Nzc, 0, 1.0, None)), warmup, reps)
+    out["x"] = _time(lambda: _lib.check(xp(cp, cp, code, Nx, Ny * Nzc, Ny * Nzc, 1, 0, 0, 1.0, None)), warmup, reps)
     return {k: round(v, 3) for k, v in out.items()}
 
 
@@ -77,7 +77,8 @@ def run_case(spec, warmup, reps, card):
     r.value.normal_()
     c = ComplexField(pm)
     field_bytes = r.value.numel() * r.value.element_size()
-    res = dict(case="r2c+c2r" if with_c2r else "r2c", Nmesh=n, dtype=dtype, path="power-of-two" if pm.pow2 else "mixed-radix")
+    path = "power-of-two" if pm.pow2 else ("bluestein" if any(pm.bluestein) else "mixed-radix")
+    res = dict(case="r2c+c2r" if with_c2r else "r2c", Nmesh=n, dtype=dtype, path=path)
     ms = _time(lambda: r.r2c(out=c), warmup, reps)
     res["r2c_ms"] = round(ms, 3)
     res["r2c_ns_per_cell"] = round(ms * 1e6 / n ** 3, 4)
@@ -88,6 +89,7 @@ def run_case(spec, warmup, reps, card):
     if with_c2r:
         ms = _time(lambda: c.c2r(out=r), warmup, reps)
         res["c2r_ms"] = round(ms, 3)
+        res["c2r_ns_per_cell"] = round(ms * 1e6 / n ** 3, 4)
         res["c2r_GBps"] = round(6 * field_bytes / (ms * 1e-3) / 1e9, 1)
         res["c2r_frac_hbm_peak"] = round(6 * field_bytes / (ms * 1e-3) / HBM_PEAK, 3)
     res.update(card)
