@@ -284,10 +284,23 @@ int nbk_slab_push_range(const void *send, void *const *peer_ptrs_host, int dtype
                         int64_t n_inner, int64_t outer_start, int64_t o0, int64_t o_cnt, int P, int rank, void *stream);
 
 /* Fourier-space resampling to another mesh size: pmesh `Field.resample`, called by MeshSource.compute(Nmesh=...)
- * (base/mesh.py:317-327).  Modes both meshes represent are copied (same integer frequency label per axis, Nyquist
- * negative), everything else in dst is zero.  Hermitian-compressed single-GPU layouts [Nx][Ny][Nz/2+1]. */
+ * (base/mesh.py:317-327).  Per axis, destination index i has the label j = i < (N+1)/2 ? i : i - N and is copied from
+ * the source mode with the same label when -m <= 2j < m, m = min(N_src, N_dst) (even m: the Nyquist label is negative);
+ * along the compressed z axis indices 0 .. m/2 map to themselves.  Everything else in dst is zero.  Any sides 2 .. 2^24-1.
+ * Hermitian-compressed single-GPU layouts [Nx][Ny][Nz/2+1]. */
 int nbk_resample_complex(const void *src, void *dst, int dtype, const int64_t *nmesh_src_host,
                          const int64_t *nmesh_dst_host, void *stream);
+/* The same rule on P > 1, where each rank holds the transposed slab [y_n][Nx][Nz/2+1] of both meshes.  The caller plans
+ * which y rows travel between which ranks and passes them as `n_ranges` (<= 32) pairs ranges_host[2i] = first local row,
+ * ranges_host[2i+1] = count, in send (pack) or receive (unpack) order; one all-to-all moves the send blocks.
+ *   pack   : send [rows listed][Nx_dst][Nz_dst/2+1] <- the listed rows of src [src_rows][Nx_src][Nz_src/2+1], remapped
+ *            in x and z.
+ *   unpack : dst [dst_rows][Nx_dst][Nz_dst/2+1]: the listed rows <- recv in order (ranges must not overlap), every
+ *            other row zero. */
+int nbk_resample_pack(const void *src, void *send, int dtype, const int64_t *nmesh_src_host, const int64_t *nmesh_dst_host,
+                      int64_t src_rows, const int64_t *ranges_host, int n_ranges, void *stream);
+int nbk_resample_unpack(const void *recv, void *dst, int dtype, const int64_t *nmesh_dst_host, int64_t dst_rows,
+                        const int64_t *ranges_host, int n_ranges, void *stream);
 
 /* elementwise helpers behind RealField/ComplexField `[...] = v`, `*= a`, `+= other`
  * (source/mesh/catalog.py:203,354,396-398; fftpower.py:128).  n counts REAL scalars. */

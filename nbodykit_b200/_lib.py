@@ -69,6 +69,8 @@ SIGNATURES = {
     "nbk_hermitian_expand": ([_vp, _vp, _i, _pi64, _vp], _i),
     "nbk_hermitian_compress": ([_vp, _vp, _i, _i64, _i64, _vp], _i),
     "nbk_resample_complex": ([_vp, _vp, _i, _pi64, _pi64, _vp], _i),
+    "nbk_resample_pack": ([_vp, _vp, _i, _pi64, _pi64, _i64, _pi64, _i, _vp], _i),
+    "nbk_resample_unpack": ([_vp, _vp, _i, _pi64, _i64, _pi64, _i, _vp], _i),
     "nbk_fft_lines_pack_range": ([_vp, _vp, _i, _i64, _i64, _i64, _i64, _i64, _i, _i, _d, _vp], _i),
     "nbk_slab_push_range": ([_vp, ctypes.POINTER(ctypes.c_void_p), _i, _i64, _i64, _i64, _i64, _i64, _i64, _i, _i, _vp], _i),
     "nbk_ylm_mul_real": ([_vp, _vp, _i, _i, _i, _pi64, _pd, _pd, _i64, _i64, _vp], _i),

@@ -113,6 +113,12 @@ class TorchComm(object):
 
     # ---- tensor collectives (device memory)
     def allreduce_tensor(self, t, op="sum"):
+        if self._backend == "gloo" and t.is_cuda:
+            # gloo reduces host memory: several ranks sharing one GPU (tests) go through a host copy
+            h = t.cpu()
+            self._dist.all_reduce(h, op=self._op(op), group=self.group)
+            t.copy_(h)
+            return t
         self._dist.all_reduce(t, op=self._op(op), group=self.group)
         return t
 
@@ -146,6 +152,13 @@ class TorchComm(object):
         return [float(v) for v in t.cpu().tolist()]
 
     def _gloo_all_to_all(self, outs, ins):
+        if any(t.is_cuda for t in outs + ins):
+            # gloo sends host memory: stage device chunks through host copies
+            h_outs = [o.cpu() for o in outs]
+            self._gloo_all_to_all(h_outs, [c.cpu() for c in ins])
+            for o, h in zip(outs, h_outs):
+                o.copy_(h)
+            return
         reqs = []
         for peer in range(self.size):
             if peer == self.rank:

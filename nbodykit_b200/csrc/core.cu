@@ -15,7 +15,7 @@ void nbk_set_error(const char *fmt, ...) {
 }
 void nbk_count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 
-extern "C" int nbk_version(void) { return 103; }
+extern "C" int nbk_version(void) { return 104; }
 extern "C" const char *nbk_last_error(void) { return g_err; }
 extern "C" int64_t nbk_launch_count(void) { return g_launches.load(); }
 

@@ -1779,8 +1779,9 @@ extern "C" int nbk_hermitian_compress(const void *full, void *comp, int dtype, i
 // compute(Nmesh=...) asks for a size other than the source's): the modes both meshes represent are copied, the rest
 // of the destination is zero (down-sampling = truncation, up-sampling = zero padding; the normalised transform keeps
 // amplitudes, so the mean is preserved).  Per axis a destination index maps to the source index with the same integer
-// frequency label, labels in [-Nmin/2, Nmin/2) (Nyquist negative, meshtools.py:150-153); along the Hermitian-compressed
-// axis indices 0 .. Nmin/2 map to themselves.  Single GPU, compressed layout [Nx][Ny][Nz/2+1].
+// frequency label j = nbk_freq(i, N) when -m <= 2j < m, m = min(N_src, N_dst): labels [-m/2, m/2) for even m (Nyquist
+// negative, meshtools.py:150-153), [-(m-1)/2, (m-1)/2] for odd m; along the Hermitian-compressed axis indices
+// 0 .. m/2 map to themselves.  Single GPU, compressed layout [Nx][Ny][Nz/2+1]; any sides.
 // ---------------------------------------------------------------------------------------------
 template <typename C>
 __global__ void __launch_bounds__(256)
@@ -1806,8 +1807,8 @@ extern "C" int nbk_resample_complex(const void *src, void *dst, int dtype, const
     NBK_CHECK_ARG(dtype == NBK_F4 || dtype == NBK_F8, "resample_complex: bad dtype %d", dtype);
     NBK_CHECK_ARG(src != nullptr && dst != nullptr && src != dst, "resample_complex: needs two distinct buffers");
     for (int d = 0; d < 3; d++)
-        NBK_CHECK_ARG(nmesh_src[d] >= 2 && nmesh_dst[d] >= 2 && nmesh_src[d] < (1 << 24) && nmesh_dst[d] < (1 << 24) &&
-                      nmesh_src[d] % 2 == 0 && nmesh_dst[d] % 2 == 0, "resample_complex: mesh sides must be even");
+        NBK_CHECK_ARG(nmesh_src[d] >= 2 && nmesh_dst[d] >= 2 && nmesh_src[d] < (1 << 24) && nmesh_dst[d] < (1 << 24),
+                      "resample_complex: mesh sides must be in 2 .. 2^24 - 1");
     int64_t rows = nmesh_dst[0] * nmesh_dst[1];
     int g = nbk_grid_for(rows * 32, 256, 8);
     cudaStream_t s = (cudaStream_t)stream;
@@ -1817,6 +1818,146 @@ extern "C" int nbk_resample_complex(const void *src, void *dst, int dtype, const
     else
         k_resample_complex<double2><<<g, 256, 0, s>>>((const double2 *)src, (double2 *)dst, (int)nmesh_src[0], (int)nmesh_src[1],
                                                       (int)nmesh_src[2], (int)nmesh_dst[0], (int)nmesh_dst[1], (int)nmesh_dst[2]);
+    NBK_LAUNCHED();
+    return NBK_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// The same resampling on P > 1, where each rank holds the transposed y slab [y_n][Nx][Nzc].  The x and z remaps are
+// local; a destination y row comes from the rank owning the source row with the same label, or from no rank.  The host
+// plans which rows travel (at most two contiguous ranges per (source, destination) pair, the labels wrap) and passes
+// them as up to NBK_RESAMPLE_MAX_RANGES (local first row, count) pairs in send / receive order.
+//   pack   : send[k] = src row of the k-th listed row, remapped in x and z to [Nx_dst][Nzc_dst]
+//   unpack : dst local row of the k-th listed row = recv[k]; rows no range lists are zero
+// ---------------------------------------------------------------------------------------------
+#define NBK_RESAMPLE_MAX_RANGES (2 * NBK_MAX_PEERS)
+struct ResampleRanges {
+    int n;
+    int first[NBK_RESAMPLE_MAX_RANGES];
+    int count[NBK_RESAMPLE_MAX_RANGES];
+};
+
+// (send slot k) -> local source row: the ranges laid end to end
+__device__ __forceinline__ int resample_slot_row(const ResampleRanges &r, int k) {
+    for (int i = 0; i < r.n; i++) {
+        if (k < r.count[i]) return r.first[i] + k;
+        k -= r.count[i];
+    }
+    return -1;
+}
+
+// local destination row -> receive slot, or -1 when no rank sends it
+__device__ __forceinline__ int resample_row_slot(const ResampleRanges &r, int row) {
+    int off = 0;
+    for (int i = 0; i < r.n; i++) {
+        if (row >= r.first[i] && row < r.first[i] + r.count[i]) return off + row - r.first[i];
+        off += r.count[i];
+    }
+    return -1;
+}
+
+template <typename C>
+__global__ void __launch_bounds__(256)
+k_resample_pack(const C *__restrict__ src, C *__restrict__ send, const ResampleRanges rr, int64_t n_slots, int sx, int sz,
+                int dx, int dz) {
+    const int szc = sz / 2 + 1, dzc = dz / 2 + 1;
+    const int mx = sx < dx ? sx : dx;
+    const int mzc = (sz < dz ? sz : dz) / 2 + 1;
+    const int64_t rows = n_slots * dx;
+    const int lane = threadIdx.x & 31;
+    const int64_t w0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t row = w0; row < rows; row += nw) {
+        const int k = (int)(row / dx), ix = (int)(row - (int64_t)k * dx);
+        const int jx = nbk_freq(ix, dx);
+        const bool ok = 2 * jx >= -mx && 2 * jx < mx;
+        const C *s = src + ((int64_t)resample_slot_row(rr, k) * sx + (jx < 0 ? jx + sx : jx)) * szc;
+        C *d = send + row * dzc;
+        for (int iz = lane; iz < dzc; iz += 32) d[iz] = (ok && iz < mzc) ? s[iz] : C{0, 0};
+    }
+}
+
+template <typename C>
+__global__ void __launch_bounds__(256)
+k_resample_unpack(const C *__restrict__ recv, C *__restrict__ dst, const ResampleRanges rr, int64_t dst_rows, int64_t row_len) {
+    const int64_t n = dst_rows * row_len;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t y = e / row_len;
+        const int k = resample_row_slot(rr, (int)y);
+        dst[e] = k >= 0 ? recv[(int64_t)k * row_len + (e - y * row_len)] : C{0, 0};
+    }
+}
+
+// checks the (first, count) pairs against [0, n_rows) and copies them into `rr`; `total` receives the listed rows
+static int resample_ranges(const char *what, const int64_t *ranges, int n_ranges, int64_t n_rows, ResampleRanges &rr,
+                           int64_t &total) {
+    NBK_CHECK_ARG(n_ranges >= 0 && n_ranges <= NBK_RESAMPLE_MAX_RANGES, "%s: %d row ranges, at most %d", what, n_ranges,
+                  NBK_RESAMPLE_MAX_RANGES);
+    NBK_CHECK_ARG(n_ranges == 0 || ranges != nullptr, "%s: ranges missing", what);
+    rr.n = n_ranges;
+    total = 0;
+    for (int i = 0; i < n_ranges; i++) {
+        const int64_t a = ranges[2 * i], c = ranges[2 * i + 1];
+        NBK_CHECK_ARG(a >= 0 && c >= 0 && a + c <= n_rows, "%s: row range %d (%lld, %lld) outside the %lld local rows", what,
+                      i, (long long)a, (long long)c, (long long)n_rows);
+        rr.first[i] = (int)a;
+        rr.count[i] = (int)c;
+        total += c;
+    }
+    return NBK_OK;
+}
+
+static int resample_sides(const char *what, const int64_t *nmesh_src, const int64_t *nmesh_dst) {
+    NBK_CHECK_ARG(nmesh_src != nullptr && nmesh_dst != nullptr, "%s: Nmesh missing", what);
+    for (int d = 0; d < 3; d++)
+        NBK_CHECK_ARG(nmesh_src[d] >= 2 && nmesh_dst[d] >= 2 && nmesh_src[d] < (1 << 24) && nmesh_dst[d] < (1 << 24),
+                      "%s: mesh sides must be in 2 .. 2^24 - 1", what);
+    return NBK_OK;
+}
+
+extern "C" int nbk_resample_pack(const void *src, void *send, int dtype, const int64_t *nmesh_src, const int64_t *nmesh_dst,
+                                 int64_t src_rows, const int64_t *ranges, int n_ranges, void *stream) {
+    NBK_CHECK_ARG(dtype == NBK_F4 || dtype == NBK_F8, "resample_pack: bad dtype %d", dtype);
+    if (resample_sides("resample_pack", nmesh_src, nmesh_dst) != NBK_OK) return NBK_ERR_ARG;
+    NBK_CHECK_ARG(src_rows >= 0 && src_rows <= nmesh_src[1], "resample_pack: %lld local rows of a side %lld",
+                  (long long)src_rows, (long long)nmesh_src[1]);
+    ResampleRanges rr;
+    int64_t slots;
+    if (resample_ranges("resample_pack", ranges, n_ranges, src_rows, rr, slots) != NBK_OK) return NBK_ERR_ARG;
+    if (slots == 0) return NBK_OK;
+    NBK_CHECK_ARG(src != nullptr && send != nullptr && src != send, "resample_pack: needs two distinct buffers");
+    int g = nbk_grid_for(slots * nmesh_dst[0] * 32, 256, 8);
+    cudaStream_t s = (cudaStream_t)stream;
+    if (dtype == NBK_F4)
+        k_resample_pack<float2><<<g, 256, 0, s>>>((const float2 *)src, (float2 *)send, rr, slots, (int)nmesh_src[0],
+                                                  (int)nmesh_src[2], (int)nmesh_dst[0], (int)nmesh_dst[2]);
+    else
+        k_resample_pack<double2><<<g, 256, 0, s>>>((const double2 *)src, (double2 *)send, rr, slots, (int)nmesh_src[0],
+                                                   (int)nmesh_src[2], (int)nmesh_dst[0], (int)nmesh_dst[2]);
+    NBK_LAUNCHED();
+    return NBK_OK;
+}
+
+extern "C" int nbk_resample_unpack(const void *recv, void *dst, int dtype, const int64_t *nmesh_dst, int64_t dst_rows,
+                                   const int64_t *ranges, int n_ranges, void *stream) {
+    NBK_CHECK_ARG(dtype == NBK_F4 || dtype == NBK_F8, "resample_unpack: bad dtype %d", dtype);
+    if (resample_sides("resample_unpack", nmesh_dst, nmesh_dst) != NBK_OK) return NBK_ERR_ARG;
+    NBK_CHECK_ARG(dst_rows >= 0 && dst_rows <= nmesh_dst[1], "resample_unpack: %lld local rows of a side %lld",
+                  (long long)dst_rows, (long long)nmesh_dst[1]);
+    ResampleRanges rr;
+    int64_t slots;
+    if (resample_ranges("resample_unpack", ranges, n_ranges, dst_rows, rr, slots) != NBK_OK) return NBK_ERR_ARG;
+    for (int i = 0; i < n_ranges; i++)
+        for (int j = 0; j < i; j++)
+            NBK_CHECK_ARG(rr.first[i] + rr.count[i] <= rr.first[j] || rr.first[j] + rr.count[j] <= rr.first[i],
+                          "resample_unpack: row ranges %d and %d overlap", j, i);
+    if (dst_rows == 0) return NBK_OK;
+    NBK_CHECK_ARG(dst != nullptr && (slots == 0 || (recv != nullptr && recv != dst)),
+                  "resample_unpack: needs two distinct buffers");
+    const int64_t row_len = nmesh_dst[0] * (nmesh_dst[2] / 2 + 1);
+    int g = nbk_grid_for(dst_rows * row_len, 256, 8);
+    cudaStream_t s = (cudaStream_t)stream;
+    if (dtype == NBK_F4) k_resample_unpack<float2><<<g, 256, 0, s>>>((const float2 *)recv, (float2 *)dst, rr, dst_rows, row_len);
+    else k_resample_unpack<double2><<<g, 256, 0, s>>>((const double2 *)recv, (double2 *)dst, rr, dst_rows, row_len);
     NBK_LAUNCHED();
     return NBK_OK;
 }

@@ -86,6 +86,54 @@ def _c2r_one_gpu(pm, cplx, real, work):
     check(pm._z_pass()(_ptr(c), _ptr(real), code, Nx * Ny, Nz, 1, 1.0, _stream()), "fft_z")
 
 
+def resample_row_plan(ny_src, ny_dst, P):
+    """which y rows a Fourier-space resample moves between the ranks of transposed slabs (rank r owns rows
+    [r N/P, (r+1) N/P) of each mesh).  A destination row with label j = nbk_freq(i, ny_dst) is copied from the source
+    row with the same label when -m <= 2j < m, m = min(ny_src, ny_dst): the rows 0 .. (m+1)/2 - 1 from themselves and
+    the last m/2 rows from the last m/2 source rows.  Returns plan[s][d], the list of (first destination row, first
+    source row, count) that source rank s sends to destination rank d, global indices, ascending: at most two ranges
+    per pair because the labels wrap."""
+    ys, yd = ny_src // P, ny_dst // P
+    m = min(ny_src, ny_dst)
+    pos, neg = (m + 1) // 2, m // 2
+    segments = [(0, 0, pos), (ny_dst - neg, ny_src - neg, neg)]     # (destination row, source row, count)
+    plan = [[[] for _ in range(P)] for _ in range(P)]
+    for s in range(P):
+        for d in range(P):
+            for d0, s0, n in segments:
+                # rows t in [0, n) with d0 + t owned by d and s0 + t owned by s
+                lo = max(0, d * yd - d0, s * ys - s0)
+                hi = min(n, (d + 1) * yd - d0, (s + 1) * ys - s0)
+                if hi > lo:
+                    plan[s][d].append((d0 + lo, s0 + lo, hi - lo))
+    return plan
+
+
+def _resample_slabs(src, dst, val, out):
+    """P > 1 Fourier-space resample of the transposed compressed slab `val` (mesh `src`) into `out` (mesh `dst`): pack
+    the rows each rank sends, one all-to-all, unpack (rows no rank sends become zero)"""
+    comm = src.comm
+    P, rank = comm.size, comm.rank
+    plan = resample_row_plan(int(src.Nmesh[1]), int(dst.Nmesh[1]), P)
+    code = _CODE[dst.typestr]
+    row = int(dst.Nmesh[0]) * dst.Nzc
+    send_r = [(s0 - src.y_start, n) for d in range(P) for _, s0, n in plan[rank][d]]
+    recv_r = [(d0 - dst.y_start, n) for s in range(P) for d0, _, n in plan[s][rank]]
+    send_rows = [sum(n for _, _, n in plan[rank][d]) for d in range(P)]
+    recv_rows = [sum(n for _, _, n in plan[s][rank]) for s in range(P)]
+    send = torch.empty((sum(send_rows), int(dst.Nmesh[0]), dst.Nzc), dtype=out.dtype, device=out.device)
+    recv = torch.empty((sum(recv_rows), int(dst.Nmesh[0]), dst.Nzc), dtype=out.dtype, device=out.device)
+    with stage("resample_pack"):
+        check(lib().nbk_resample_pack(_ptr(val), _ptr(send), code, src._nmesh_c, dst._nmesh_c, src.y_n,
+                                      iarr([v for r in send_r for v in r]), len(send_r), _stream()), "nbk_resample_pack")
+    with stage("resample_alltoall"):
+        comm.all_to_all_single(torch.view_as_real(recv).view(-1), torch.view_as_real(send).view(-1),
+                               [2 * row * n for n in recv_rows], [2 * row * n for n in send_rows])
+    with stage("resample_unpack"):
+        check(lib().nbk_resample_unpack(_ptr(recv), _ptr(out), code, dst._nmesh_c, dst.y_n,
+                                        iarr([v for r in recv_r for v in r]), len(recv_r), _stream()), "nbk_resample_unpack")
+
+
 def current_device():
     if not torch.cuda.is_available():
         raise _lib.NbkError("nbodykit_b200 needs a CUDA device (sm_90a, H100); there is no CPU fallback")
@@ -806,15 +854,35 @@ class Field(object):
 
     def resample(self, out):
         """the field on the mesh of `out` by Fourier-space resampling (pmesh `Field.resample`, base/mesh.py:317-327):
-        common modes are copied, the others are zero; real fields go through r2c / c2r.  Single GPU."""
+        common modes are copied, the others are zero (the rule of nbk_resample_complex, any sides); real fields go through
+        r2c / c2r.  Complex-dtype meshes are resampled through their Hermitian-compressed half.  On P > 1 both meshes
+        need Nx and Ny divisible by P, as every mesh there does."""
         pm, dst = self.pm, out.pm
-        if pm.comm.size > 1 or pm.cplx or dst.cplx:
-            raise NotImplementedError("Fourier-space resampling is implemented for one GPU and Hermitian-compressed meshes")
+        if dst.comm.size != pm.comm.size:
+            raise ValueError("resample: both fields must live on the same communicator")
         src_c = self if isinstance(self, BaseComplexField) else self.r2c()
         dst_c = out if isinstance(out, BaseComplexField) else ComplexField(dst)
-        val = src_c.value if pm.typestr == dst.typestr else src_c.value.to(dst_c.value.dtype)
-        check(lib().nbk_resample_complex(_ptr(val), _ptr(dst_c.value), _CODE[dst.typestr], pm._nmesh_c, dst._nmesh_c, _stream()),
-              "nbk_resample_complex")
+        val = src_c.value
+        if pm.cplx:
+            Sx, Sy, Sz = [int(v) for v in pm.Nmesh]
+            half = torch.empty((Sx, Sy, Sz // 2 + 1), dtype=val.dtype, device=val.device)
+            check(lib().nbk_hermitian_compress(_ptr(val), _ptr(half), _CODE[pm.typestr], Sx * Sy, Sz, _stream()),
+                  "nbk_hermitian_compress")
+            val = half
+        if pm.typestr != dst.typestr:
+            val = val.to(dst_c.value.dtype)
+        target = dst_c.value
+        if dst.cplx:
+            Dx, Dy, Dz = [int(v) for v in dst.Nmesh]
+            target = torch.empty((Dx, Dy, Dz // 2 + 1), dtype=target.dtype, device=target.device)
+        if pm.comm.size == 1:
+            check(lib().nbk_resample_complex(_ptr(val), _ptr(target), _CODE[dst.typestr], pm._nmesh_c, dst._nmesh_c,
+                                             _stream()), "nbk_resample_complex")
+        else:
+            _resample_slabs(pm, dst, val, target)
+        if dst.cplx:
+            check(lib().nbk_hermitian_expand(_ptr(target), _ptr(dst_c.value), _CODE[dst.typestr], dst._nmesh_c, _stream()),
+                  "nbk_hermitian_expand")
         if isinstance(out, RealField):
             dst_c.c2r(out=out)
         out.attrs = dict(self.attrs)
@@ -841,10 +909,16 @@ class RealField(Field):
     def preview(self, Nmesh=None, axes=None):
         """the field, optionally summed over the axes NOT listed in `axes`, as a numpy array on every rank (pmesh
         `Field.preview`; fftpower.py:432).  The reduction over dropped axes runs on the device; only the projected
-        array crosses PCIe."""
+        array crosses PCIe.  `Nmesh` other than the field's first resamples it in Fourier space (`resample`) onto a mesh
+        of that size on the same GPUs, so on P > 1 GPUs Nmesh[0] and Nmesh[1] must be divisible by P."""
         pm = self.pm
         if Nmesh is not None and any(numpy.ones(3, 'i8') * Nmesh != pm.Nmesh):
-            raise NotImplementedError("preview at a different resolution is not implemented")
+            N = numpy.ones(3, 'i8') * Nmesh
+            P = pm.comm.size
+            if N[0] % P or N[1] % P:
+                raise ValueError("preview(Nmesh=%s) on %d GPUs: Nmesh[0] and Nmesh[1] must be divisible by the number of "
+                                 "GPUs, as the field is resampled onto a mesh of that size" % (list(N), P))
+            return self.resample(RealField(pm.reshape(Nmesh=N))).preview(axes=axes)
         if axes is None:
             axes = [0, 1, 2]
         axes = [axes] if numpy.isscalar(axes) else list(axes)
