@@ -378,7 +378,10 @@ __device__ __forceinline__ int make_record(const PT *x, const TileGeom &tg, unsi
         int ri = __double2loint(r);
         double rf = r - K;                                  // rint(a)
         if (rf > a) { rf -= 1.0; ri -= 1; }                 // floor(a)
-        u[d] = (unsigned)__double2loint(__dadd_rz((a - rf) * 4294967296.0, 4503599627370496.0));
+        // a - floor(a) rounds to 1.0 for a in (-2^-54, 0): saturate as the slow path's conversion does (2^32 would wrap
+        // to a zero fraction and move the whole weight one cell down)
+        const double fr = a - rf;
+        u[d] = fr < 1.0 ? (unsigned)__double2loint(__dadd_rz(fr * 4294967296.0, 4503599627370496.0)) : 0xffffffffu;
         int cc = ri + WinOff<SUP>::B;                       // one period of wrap here, anything further in the slow path
         if (cc < 0) cc += tg.gm.n[d];
         else if (cc >= tg.gm.n[d]) cc -= tg.gm.n[d];
@@ -426,7 +429,11 @@ __device__ __forceinline__ int make_record_pow2(const float *x, const TileGeom &
         const float g = x[d] * ft.sc[d];                       // exact
         ok = ok && (fabsf(g) < 4194304.0f);                    // false for NaN / inf as well; far outside: slow path
         const float f = floorf(g);
-        unsigned u28 = (unsigned)((g - f) * 268435456.0f);     // (g - f) exact; cvt truncates: floor(frac * 2^28)
+        // (g - f) is exact except for g in (-2^-25, 0), where it rounds to 1.0: those take the f8 path, which rounds
+        // g + A as the contract does
+        const float fr = g - f;
+        ok = ok && (fr < 1.0f);
+        unsigned u28 = (unsigned)(fr * 268435456.0f);          // cvt truncates: floor(frac * 2^28)
         int ci = (int)f;
         if (WinOff<SUP>::A != 0.f) {
             u28 += 1u << 27;
@@ -451,13 +458,16 @@ __device__ __forceinline__ int tile_fast(const PT *x, const TileGeom &tg, const 
     ok = sizeof(PT) == 4;
     int c[3] = {0, 0, 0};
     if (sizeof(PT) == 4 && ft.pow2) {
-        // N/L a power of two: g = x * scale (and g + 1/2) is exact in float32, so floor(g) IS the f8 result -- no margin test
+        // N/L a power of two: g = x * scale is exact in float32, so floor(g) IS the f8 result -- no margin test.  The
+        // 1/2 of NNB / TSC is a carry on the exact fraction, as in make_record_pow2: g + 1/2 rounded in float32 is not
+        // exact below 1/2 (g = 1/2 - 2^-25 gives 1.0), which put the count pass one cell -- for TSC one tile -- off
 #pragma unroll
         for (int d = 0; d < 3; d++) {
-            float g = (float)x[d] * ft.sc[d];
-            if (WinOff<SUP>::A != 0.f) g += WinOff<SUP>::A;
+            const float g = (float)x[d] * ft.sc[d];
             ok = ok && (fabsf(g) < 4194304.0f);                  // also false for NaN / inf
-            c[d] = __float2int_rd(g) + WinOff<SUP>::B;
+            int ci = __float2int_rd(g);
+            if (WinOff<SUP>::A != 0.f && g - floorf(g) >= 0.5f) ci += 1;
+            c[d] = ci + WinOff<SUP>::B;
             ok = ok && ((unsigned)c[d] < (unsigned)tg.gm.n[d]);
         }
     } else if (sizeof(PT) == 4) {
