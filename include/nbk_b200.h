@@ -138,7 +138,9 @@ int nbk_sum_w_w2(const void *w, int dtype, int64_t n, double *out2, void *stream
 
 /* RealField.r2c / ComplexField.c2r (base/mesh.py:228,237; source/mesh/catalog.py:341-351).
  * Forward is normalised by 1/(Nx*Ny*Nz), backward unnormalised (source/mesh/array.py:36-37).
- * Single-GPU whole-mesh transforms; real [Nx][Ny][Nz], cplx [Nx][Ny][Nzc].  Out of place. */
+ * Single-GPU whole-mesh transforms; real [Nx][Ny][Nz], cplx [Nx][Ny][Nzc].  Out of place.
+ * Limits: every side a power of two, Nz >= 4; Nx, Ny <= 8192 and Nz <= 16384 in f4, Nx, Ny <= 4096 and Nz <= 8192 in
+ * f8 (one CTA holds a whole line in shared memory).  The same line limits hold for the slab passes below. */
 int nbk_r2c(const void *real, void *cplx, int dtype, const int64_t *nmesh_host, double extra_scale,
             void *stream); /* cplx = extra_scale * FFT(real) / prod(N): folds e.g. the 1/nbar of catalog.py:394-398 */
 int nbk_c2r(const void *cplx, void *real, int dtype, const int64_t *nmesh_host, void *work,

@@ -1205,6 +1205,9 @@ static int ilog2(int64_t n) {
     return l;
 }
 static bool is_pow2(int64_t n) { return n > 0 && (n & (n - 1)) == 0; }
+// longest power-of-two complex line (x / y lines; the z pass runs Nz/2-point lines): one CTA keeps a whole line of
+// at least N (B + 2) complex values, B >= 1, in its 227 KB of shared memory -- 8192 points in f4, 4096 in f8
+static int64_t pow2_max_line(int dtype) { return dtype == NBK_F4 ? 8192 : 4096; }
 
 // pick the number of side-by-side lines: >= 64 B contiguous runs, tile <= ~96 KB (2 CTAs / SM)
 static int pick_B(int N, int csize, int64_t n_inner) {
@@ -1413,8 +1416,9 @@ static int launch_lines(const void *data, void *dst, int N, int64_t line_stride,
 extern "C" int nbk_fft_lines(void *cplx, int dtype, int64_t n_line, int64_t line_stride, int64_t n_inner,
                              int64_t n_outer, int64_t outer_stride, int inverse, double scale, void *stream) {
     NBK_CHECK_ARG(dtype == NBK_F4 || dtype == NBK_F8, "fft_lines: bad dtype %d", dtype);
-    NBK_CHECK_ARG(is_pow2(n_line) && n_line <= 8192, "fft_lines: line length %lld is not a supported power of two",
-                  (long long)n_line);
+    NBK_CHECK_ARG(is_pow2(n_line) && n_line <= pow2_max_line(dtype),
+                  "fft_lines: line length %lld is not a power of two of at most %lld points", (long long)n_line,
+                  (long long)pow2_max_line(dtype));
     if (n_inner <= 0 || n_outer <= 0) return NBK_OK;
     cudaStream_t s = (cudaStream_t)stream;
     if (dtype == NBK_F4)
@@ -1427,7 +1431,9 @@ extern "C" int nbk_fft_lines_oop(const void *src, void *dst, int dtype, int64_t 
                                  int64_t n_inner, int64_t n_outer, int64_t outer_stride, int inverse, double scale,
                                  void *stream) {
     NBK_CHECK_ARG(dtype == NBK_F4 || dtype == NBK_F8, "fft_lines_oop: bad dtype %d", dtype);
-    NBK_CHECK_ARG(is_pow2(n_line) && n_line >= 2 && n_line <= 8192, "fft_lines_oop: line length %lld unsupported", (long long)n_line);
+    NBK_CHECK_ARG(is_pow2(n_line) && n_line >= 2 && n_line <= pow2_max_line(dtype),
+                  "fft_lines_oop: line length %lld unsupported (a power of two of at most %lld points)", (long long)n_line,
+                  (long long)pow2_max_line(dtype));
     if (n_inner <= 0 || n_outer <= 0) return NBK_OK;
     cudaStream_t s = (cudaStream_t)stream;
     if (dtype == NBK_F4)
@@ -1567,9 +1573,11 @@ static int launch_z(const void *in, void *out, int64_t rows, int Nz, bool forwar
 
 static int check_dims(const char *who, int dtype, int64_t Nx, int64_t Ny, int64_t Nz) {
     NBK_CHECK_ARG(dtype == NBK_F4 || dtype == NBK_F8, "%s: bad dtype %d", who, dtype);
-    NBK_CHECK_ARG(is_pow2(Nx) && is_pow2(Ny) && is_pow2(Nz) && Nz >= 4 && Nx <= 8192 && Ny <= 8192 && Nz <= 16384,
-                  "%s: Nmesh (%lld,%lld,%lld) unsupported: each side must be a power of two (Nz >= 4)", who,
-                  (long long)Nx, (long long)Ny, (long long)Nz);
+    const int64_t ml = pow2_max_line(dtype);
+    NBK_CHECK_ARG(is_pow2(Nx) && is_pow2(Ny) && is_pow2(Nz) && Nz >= 4 && Nx <= ml && Ny <= ml && Nz <= 2 * ml,
+                  "%s: Nmesh (%lld,%lld,%lld) unsupported: each side must be a power of two (Nz >= 4), Nx and Ny at "
+                  "most %lld and Nz at most %lld in %s", who, (long long)Nx, (long long)Ny, (long long)Nz,
+                  (long long)ml, (long long)(2 * ml), dtype == NBK_F4 ? "f4" : "f8");
     return NBK_OK;
 }
 
@@ -1976,7 +1984,9 @@ extern "C" int nbk_fft_lines_pack_range(const void *src, void *send, int dtype, 
                                         int64_t n_outer, int64_t o0, int64_t o_cnt, int P, int inverse, double scale,
                                         void *stream) {
     NBK_CHECK_ARG(dtype == NBK_F4 || dtype == NBK_F8, "fft_lines_pack_range: bad dtype %d", dtype);
-    NBK_CHECK_ARG(is_pow2(n_line) && n_line >= 2 && n_line <= 8192, "fft_lines_pack_range: line length %lld unsupported", (long long)n_line);
+    NBK_CHECK_ARG(is_pow2(n_line) && n_line >= 2 && n_line <= pow2_max_line(dtype),
+                  "fft_lines_pack_range: line length %lld unsupported (a power of two of at most %lld points)",
+                  (long long)n_line, (long long)pow2_max_line(dtype));
     NBK_CHECK_ARG(P >= 1 && P <= NBK_MAX_PEERS && n_line % P == 0, "fft_lines_pack_range: bad peer count %d", P);
     NBK_CHECK_ARG(o0 >= 0 && o_cnt >= 0 && o0 + o_cnt <= n_outer, "fft_lines_pack_range: bad sub-range");
     if (n_inner <= 0 || o_cnt <= 0) return NBK_OK;

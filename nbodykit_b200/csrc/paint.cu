@@ -274,6 +274,7 @@ struct TileGeom {
     int G;            // ghost reach below the slab in x (0 when the slab is the whole mesh)
     int nt[3];        // tiles per axis
     int R;            // region edge = TILE + support - 1 (+1 when a half-cell shifted mesh is painted)
+    int shifted;      // a half-cell shifted mesh is painted from the records (see shift_carry)
     int ntiles;
     int full;         // the slab is the whole mesh (single GPU): no ghost / ownership logic
 };
@@ -329,6 +330,16 @@ __device__ __forceinline__ void pack_record(const unsigned *u, const int *c, con
     rec[2] = (u[2] >> 4) | ((unsigned)(c[2] & (TILE - 1)) << 28);
 }
 
+// The shifted mesh takes frac + 1/2 in fixed point, while the contract rounds in f8: g' = fl(a + 1/2) (po.grid_coords,
+// the direct path).  Where fl(a + 1/2) rounds up onto the next integer (a + 1/2 below it by at most half an ulp: e.g.
+// a = 1/2 - 2^-54) the contract's stencil starts one cell higher than the carry of the truncated fraction gives, and
+// the shifted mesh would put a 2^-28 weight on a cell outside it.  There the record stores frac = 1/2 exactly, so the
+// carry happens; the unshifted weights move by at most half an ulp of a + 1/2 (< 2^-28 for |g| < 2^24), within the
+// truncation error the record already allows.
+__device__ __forceinline__ unsigned shift_carry(unsigned u, double a, double f, const TileGeom &tg) {
+    return (tg.shifted && u < 0x80000000u && (a + 0.5) - f >= 1.0) ? 0x80000000u : u;
+}
+
 // exact leftmost cell + fixed-point fraction (the arithmetic of Window<SUP>::eval on the unshifted g).
 // Slow path: any magnitude, 64-bit cell arithmetic.
 struct RecTile { unsigned r[3]; int tile; };
@@ -346,7 +357,7 @@ __device__ __noinline__ RecTile make_record_slow3(PT x0, PT x1, PT x2, const Til
         if (!isfinite(g)) return o;
         double a = g + (double)WinOff<SUP>::A;
         double f = floor(a);
-        u[d] = __double2uint_rz((a - f) * 4294967296.0);
+        u[d] = shift_carry(__double2uint_rz((a - f) * 4294967296.0), a, f, tg);
         c[d] = wrap((long long)f + WinOff<SUP>::B, tg.gm.n[d]);
     }
     pack_record(u, c, tg, o.r);
@@ -388,7 +399,8 @@ __device__ __forceinline__ int make_record(const PT *x, const TileGeom &tg, unsi
         fast = fast && ((unsigned)cc < (unsigned)tg.gm.n[d]);
         c[d] = cc;
     }
-    if (!fast) return make_record_slow<SUP, PT>(x, tg, rec);
+    // a half-cell shifted mesh takes the slow path, which applies shift_carry (the unshifted paints keep this path lean)
+    if (!fast || tg.shifted) return make_record_slow<SUP, PT>(x, tg, rec);
     pack_record(u, c, tg, rec);
     return tile_from_cells(c, tg);      // the tile the bucketing pass counted this particle in (both are exact)
 }
@@ -418,7 +430,8 @@ static FastTile make_fast_tile(const TileGeom &tg) {      // host side: passed t
 // float32 positions on a mesh whose N/L is a power of two (every benchmark box: L = 2 N): g = x * scale is EXACT in
 // float32, so the leftmost cell and the 28-bit truncated fraction follow from float32 / integer arithmetic alone and
 // are bit-identical to the f8 path (same real number, same truncation): ~8 instructions per axis instead of ~25.
-// frac(g + 1/2) (TSC, NNB) is formed in fixed point: + 2^27 with the carry moving to the cell.
+// frac(g + 1/2) (TSC, NNB) is formed in fixed point: + 2^27 with the carry moving to the cell.  A float32 value plus 1/2
+// is exact in f8, so the shifted mesh's carry already is the contract's rounding here (no shift_carry needed).
 template <int SUP>
 __device__ __forceinline__ int make_record_pow2(const float *x, const TileGeom &tg, const FastTile &ft, unsigned *rec, bool &ok) {
     unsigned u[3];
@@ -1438,6 +1451,7 @@ static int make_tile_geom(const PaintGeom &gm, int sup, bool shifted, TileGeom &
     tg.G = (gm.x_n == gm.n[0]) ? 0 : sup + 1;
     tg.full = (gm.x_n == gm.n[0] && gm.x_start == 0) ? 1 : 0;
     tg.R = TILE + sup - 1 + (shifted ? 1 : 0);
+    tg.shifted = shifted ? 1 : 0;
     tg.nt[0] = (gm.x_n + tg.G + TILE - 1) / TILE;
     tg.nt[1] = (gm.n[1] + TILE - 1) / TILE;
     tg.nt[2] = (gm.n[2] + TILE - 1) / TILE;

@@ -316,8 +316,9 @@ class ParticleMesh(object):
         self.y_start = self.comm.rank * self.y_n
         self.Nzc = Nz if self.cplx else Nz // 2 + 1      # stored length of the last axis of a ComplexField
         self.transposed = P > 1
-        # every side a power of two: the radix-8 kernels (and, with P > 1, the NVLink peer transpose); otherwise the
-        # mixed-radix passes, whose entry points check the sizes they take
+        # every side a power of two: the radix-8 kernels (and, with P > 1, the NVLink peer transpose), which take lines
+        # up to 8192 points in f4 and 4096 in f8 (Nz up to twice that); otherwise the mixed-radix passes.  The entry
+        # points check the sizes they take
         self.pow2 = all(n > 0 and n & (n - 1) == 0 for n in (Nx, Ny, Nz))
         # of those, the axes (x, y, z) whose side has a prime factor above 7 take the Bluestein passes instead
         self.bluestein = tuple(not _smooth7(n) for n in (Nx, Ny, Nz))
@@ -1006,6 +1007,9 @@ class RealField(Field):
             with stage("r2c"):
                 check(lib().nbk_r2c(_ptr(self.value), _ptr(out.value), code, pm._nmesh_c, float(scale), _stream()), "nbk_r2c")
         else:
+            # the x lines run last, after the z / y passes and the exchange: check their length before any launch (a
+            # call without work only validates the arguments)
+            check(lib().nbk_fft_lines(None, code, Nx, 0, 0, 0, 0, 0, 1.0, None), "fft_lines(x)")
             Nzc = pm.Nzc
             work = torch.empty((pm.x_n, Ny, Nzc), dtype=out.value.dtype, device=out.value.device)
             st = pm._peer_stage()

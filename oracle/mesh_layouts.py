@@ -1,11 +1,14 @@
 """
-TEST INFRASTRUCTURE -- helpers of tests/test_gpu_mesh_layouts.py (never imported by the product):
+TEST INFRASTRUCTURE -- helpers of tests/test_gpu_mesh_layouts.py and tests/test_gpu_slab_route.py (never imported by
+the product):
 
   * the slab layouts the Fourier- and real-space kernels take, as P virtual ranks of one array: the transposed y slabs
     [y_n][Nx][Nzc] that the slab FFT leaves on every GPU when P > 1, and the real x slabs [x_n][Ny][Nz];
   * float64 references on full (uncompressed) meshes where pmesh_oracle only knows the Hermitian half;
   * particle positions on and around the cell boundaries of the paint index arithmetic, and the CPU checks that show
     the positions do land there;
+  * the particle routing between x slabs: positions around the slab edges and the route's float32 rejection edges, and
+    the ranks a paint / readout stencil touches;
   * the fixed-point contract of the tiled paint: the scale the kernel derives from the masses, the exact NNB result it
     implies, and a per-cell error bound for the other windows.
 """
@@ -183,6 +186,88 @@ def fast_tile_needs_f8(x, n, l, resampler):
     fr = (g - np.floor(g)).astype(f4)
     lim = f4(0.5) - (f4(3e-7) * f4(n + 2) + f4(1e-6))
     return ~(np.abs(fr - f4(0.5)) < lim)
+
+
+# ----------------------------------------------------------------------------------------------
+# particle routing between x slabs (csrc/route.cu)
+# ----------------------------------------------------------------------------------------------
+def route_margin(Nx):
+    """the float32 margin of the route's rejection test, in cells: 1e-3 + 4e-7 Nx, in float32 as a multiply then an add
+    (csrc/route.cu is compiled with --fmad=false, so the device does not contract them into an FMA either; the +-3
+    float32 ulp neighbours of slab_edge_values would straddle an edge one ulp away as well)"""
+    f4 = np.float32
+    return f4(1e-3) + f4(4e-7) * f4(Nx)
+
+
+def route_reject_edges(Nx, P, s):
+    """float32 grid coordinates (in_lo, in_hi) of every rank: a particle with in_lo < fl32(x) fl32(N/L) < in_hi is
+    rejected in float32 (never examined in f8)"""
+    f4 = np.float32
+    x_n, m = Nx // P, route_margin(Nx)
+    return [(f4(r * x_n) + f4(s) + m, f4((r + 1) * x_n) - f4(s) - m) for r in range(P)]
+
+
+def slab_edge_targets(Nx, P, smoothings):
+    """the grid coordinates b + d the slab-edge generator targets: every slab boundary b = r x_n (r = 0 .. P, the seam
+    at 0 = Nx included) with d in {-s-1, -s, -1/2, 0, 1/2, s, s+1} for every smoothing s"""
+    x_n = Nx // P
+    t = set()
+    for r in range(P + 1):
+        for s in smoothings:
+            for d in (-s - 1, -s, -0.5, 0.0, 0.5, s, s + 1):
+                t.add(float(r * x_n + d))
+    return sorted(t)
+
+
+def slab_edge_values(Nx, L, P, smoothings, dtype, k=3):
+    """x coordinates (in `dtype`) around the slab edges of the routing: every target of slab_edge_targets and every
+    float32 rejection edge of route_reject_edges, each with its +-0..k ulp neighbours (float32 ulps for the rejection
+    edges, which live in float32); the seam targets moved 1 .. 3 box lengths out on both sides; +0 and -0"""
+    L = float(L)
+    sc32 = np.float32(float(Nx) / L)
+    vals = []
+    targets = slab_edge_targets(Nx, P, smoothings)
+    for g in targets:
+        vals += _ulp_neighbours(g * L / Nx, dtype, k)
+    for s in smoothings:
+        for lo, hi in route_reject_edges(Nx, P, s):
+            for e in (lo, hi):
+                # the float32 x whose fl32(x * fl32(N/L)) is nearest to the edge, and its float32 neighbours
+                x = np.float32(np.float64(e) / np.float64(sc32))
+                vals += [np.asarray(v, dtype=dtype) for v in _ulp_neighbours(x, np.float32, k)]
+    seam = [g for g in targets if abs(g) <= max(smoothings) + 1]
+    for j in (-3, -2, -1, 1, 2, 3):
+        for g in seam:
+            vals += _ulp_neighbours((g + j * Nx) * L / Nx, dtype, 1)
+    out = np.unique(np.asarray(vals, dtype=dtype))
+    return np.append(out, np.asarray([0.0, -0.0], dtype=dtype))
+
+
+def slab_edge_positions(N, L, P, smoothings, dtype, n_uniform=5000, seed=0):
+    """positions whose x is a slab_edge_values value (y, z uniform in the box) followed by n_uniform uniform
+    particles.  Returns (pos, number of edge rows)"""
+    rng = np.random.RandomState(seed)
+    L = np.asarray(L, dtype="f8")
+    v = slab_edge_values(int(N[0]), L[0], P, smoothings, dtype)
+    edge = (rng.uniform(0, 1, size=(len(v), 3)) * L).astype(dtype)
+    edge[:, 0] = v
+    uni = (rng.uniform(0, 1, size=(n_uniform, 3)) * L).astype(dtype)
+    return np.concatenate([edge, uni]), len(v)
+
+
+def stencil_ranks(pos, N, L, P, resampler, shifts):
+    """bitmask (int64) of the ranks of P x slabs that own a plane the window stencil of each particle touches, at any
+    of `shifts` -- from the exact paint / readout cell arithmetic (po.grid_coords, po.window_1d), not from the route"""
+    Nx = int(N[0])
+    x_n = Nx // P
+    sup = po.SUPPORT[resampler]
+    mask = np.zeros(len(pos), dtype="i8")
+    for shift in shifts:
+        g = po.grid_coords(pos, N, L, shift)[:, 0]
+        i0 = po.window_1d(g, resampler)[0]
+        for j in range(sup):
+            mask |= np.left_shift(1, ((i0 + j) % Nx) // x_n).astype("i8")
+    return mask
 
 
 # ----------------------------------------------------------------------------------------------

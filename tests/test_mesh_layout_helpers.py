@@ -131,3 +131,48 @@ def test_project_sums_anti_matches_full_mesh():
     khat, mhat = ml.mirror_dirs(N, L)
     for d in range(3):
         np.testing.assert_array_equal(mhat[d], -khat[d])
+
+
+# ---- the slab-edge generator of tests/test_gpu_slab_route.py --------------------------------------------------------
+ROUTE_GEOMS = [((48, 32, 32), 3), ((40, 32, 32), 8), ((32, 32, 32), 8), ((64, 16, 16), 32)]
+SMOOTHINGS = (0.5, 1.0, 1.5, 2.0, 2.5, 3.0, 4.0)
+
+
+@pytest.mark.parametrize("NP", ROUTE_GEOMS, ids=lambda g: "%s-P%d" % g if isinstance(g, tuple) else str(g))
+@pytest.mark.parametrize("lx", [100., 24.])
+@pytest.mark.parametrize("dtype", ["f4", "f8"])
+def test_slab_edge_positions_reach_both_sides(NP, lx, dtype):
+    """every slab-edge target b + d is straddled in exact f8 grid units, every float32 rejection edge in the route's
+    float32 arithmetic, and the seam images 1 .. 3 box lengths out are present"""
+    N, P = NP
+    Nx = N[0]
+    L = (lx, 30., 30.)
+    pos, n_edge = ml.slab_edge_positions(N, L, P, SMOOTHINGS, dtype)
+    assert pos.dtype == np.dtype(dtype) and n_edge > 0
+    x = pos[:n_edge, 0]
+    g = x.astype("f8") * (Nx / lx)
+    for t in ml.slab_edge_targets(Nx, P, SMOOTHINGS):
+        near = np.abs(g - t) < 1e-3
+        assert (g[near] < t).any() and (g[near] >= t).any(), "target %g" % t
+    g32 = x.astype(np.float32) * np.float32(Nx / lx)
+    for s in SMOOTHINGS:
+        for lo, hi in ml.route_reject_edges(Nx, P, s):
+            for e in (lo, hi):
+                near = np.abs(g32.astype("f8") - float(e)) < 1e-3
+                assert (g32[near] > e).any() and (g32[near] <= e).any(), "edge %g (s=%g)" % (e, s)
+    for j in (-3, -1, 1, 3):
+        assert (np.abs(g - j * Nx) < 1e-3).any()
+    assert (np.signbit(x) & (x == 0)).any() and (~np.signbit(x) & (x == 0)).any()
+
+
+def test_route_margin_and_stencil_ranks():
+    assert ml.route_margin(1024) == np.float32(1e-3) + np.float32(4e-7) * np.float32(1024)
+    N, L, P = (16, 4, 4), (16., 4., 4.), 4                      # x_n = 4, one cell per unit length
+    x = np.array([3.5, 3.99, 0.2, 15.7, 7.5, 8.0])
+    pos = np.stack([x, np.ones_like(x), np.ones_like(x)], axis=1)
+    # cic: cells floor(g), floor(g) + 1; shift 0.5 moves both up by one when frac(g) >= 1/2
+    assert ml.stencil_ranks(pos, N, L, P, "cic", [0.0]).tolist() == [0b11, 0b11, 0b1, 0b1001, 0b110, 0b100]
+    assert ml.stencil_ranks(pos, N, L, P, "cic", [0.0, 0.5]).tolist() == [0b11, 0b11, 0b1, 0b1001, 0b110, 0b100]
+    # nnb: the nearest cell floor(g + 1/2); pcs: floor(g) - 1 .. floor(g) + 2
+    assert ml.stencil_ranks(pos, N, L, P, "nnb", [0.0]).tolist() == [0b10, 0b10, 0b1, 0b1, 0b100, 0b100]
+    assert ml.stencil_ranks(pos, N, L, P, "pcs", [0.0]).tolist() == [0b11, 0b11, 0b1001, 0b1001, 0b110, 0b110]
