@@ -304,6 +304,67 @@ int nbk_resample_pack(const void *src, void *send, int dtype, const int64_t *nme
 int nbk_resample_unpack(const void *recv, void *dst, int dtype, const int64_t *nmesh_dst_host, int64_t dst_rows,
                         const int64_t *ranges_host, int n_ranges, void *stream);
 
+/* Friends-of-friends groups (algorithms/fof.py: `_fof_local`, `_fof_merge`, `_assign_labels`, `centerofmass`,
+ * `fof_catalog`).  Two particles are friends when d^2 = (dx^2 + dy^2) + dz^2 <= b^2, evaluated in double from the stored
+ * positions (no FMA); periodic: positions wrapped as numpy's `pos % L` in their own dtype, per-axis |d| -> min(|d|, L - |d|).
+ * Rows: n < 2^32.  The cell grid has ncell_host[d] cells of side box[d] / ncell[d] <= b / sqrt(3) per axis (non-periodic:
+ * starting at origin_host, box = extent); cells are 63-bit keys (x-major).
+ *   cell_keys   : keys[n] (int64) of every particle.
+ *   sort        : stable LSD radix sort of `keys` (uint64, key_bytes 8, or uint32, key_bytes 4; bits [0, end_bit)) carrying
+ *                 the row index (uint32, filled by the call) along; n < 2^31.  keys/keys_alt and rows/rows_alt are the two
+ *                 halves of a double buffer; *result_in_alt (host) says which one holds the result.  work: device scratch
+ *                 of nbk_fof_sort_workspace(n, key_bytes) bytes.
+ *   sorted_pos  : sorted_pos[i] = (wrapped) pos[perm[i]], perm = the key sort permutation (uint32).
+ *   compact     : occupied cells of the sorted keys.  compact_count: *ncells (device int64); compact_write:
+ *                 cell_start[0..ncells] (uint32, last entry = n), cell_key[ncells].  work: device
+ *                 int64[nbk_fof_compact_workspace(n)], the same for both calls.
+ *   link        : union-find over the cells: parent[ncells] (uint32, every entry its root on return), cell_min[ncells] (smallest
+ *                 global id in the cell; at a root, of its component).  Global id of row r: gid[r], or gid_base + r when gid is
+ *                 NULL.  Every pair of cells within reach is united when one particle pair links.
+ *   finalize    : per row r: row_root[r] = root cell, minid[r] = smallest global id of its group (minid may be NULL).
+ *   lower       : per row, minid[r] <- the smallest new_minid[] over the rows of its root (the `_fof_merge` step on one rank);
+ *                 *changed (device uint64, accumulated) += rows whose value changed.  root_min: device int64[ncells] scratch.
+ *   root_counts : counts[row_root[r]] += 1 (device uint64[ncells], zero first).
+ *   label_rows  : labels[r] = cell_label[row_root[r]] as int32 (label_bytes 4) or int64 (8).
+ *   segment_reduce : rows ordered by label (`order`, uint32), split into chunks: chunk k = sorted rows [chunk_first[k], chunk_first[k+1])
+ *                 of label chunk_label[k]; label l owns chunks [label_chunk[l], label_chunk[l+1]).  Fixed-order reduction into
+ *                 out[nlabels][4] (partial: device double[nchunks][4] scratch):
+ *                   NBK_FOF_RED_MIN  per-axis minimum of a [n][3] column        (slot 3: rows)
+ *                   NBK_FOF_RED_MAX  maximum of a [n] column in slot 0          (slot 3: rows)
+ *                   NBK_FOF_RED_SUM  per-axis sum of col - ref[l] (ref NULL: col), wrapped into [-L/2, L/2) when periodic
+ *                                    and ref is given; slot 3: rows
+ *                 mask != NULL restricts MIN / SUM to rows with mask[r] >= thresh[l]. */
+#define NBK_FOF_RED_MIN 0
+#define NBK_FOF_RED_MAX 1
+#define NBK_FOF_RED_SUM 2
+int nbk_fof_cell_keys(const void *pos, int pos_dtype, int64_t n, int periodic, const double *box_host,
+                      const double *origin_host, const int64_t *ncell_host, double b, int64_t *keys, void *stream);
+int64_t nbk_fof_sort_workspace(int64_t n, int key_bytes);
+int nbk_fof_sort(void *keys, void *keys_alt, uint32_t *rows, uint32_t *rows_alt, int64_t n, int key_bytes, int end_bit,
+                 void *work, int64_t work_bytes, int *result_in_alt, void *stream);
+int nbk_fof_sorted_pos(const void *pos, int pos_dtype, int64_t n, const uint32_t *perm, int periodic,
+                       const double *box_host, void *sorted_pos, void *stream);
+int64_t nbk_fof_compact_workspace(int64_t n);
+int nbk_fof_compact_count(const int64_t *sorted_keys, int64_t n, int64_t *work, int64_t work_len, int64_t *ncells,
+                          void *stream);
+int nbk_fof_compact_write(const int64_t *sorted_keys, int64_t n, const int64_t *work, int64_t work_len,
+                          uint32_t *cell_start, int64_t *cell_key, void *stream);
+int nbk_fof_link(const void *sorted_pos, int pos_dtype, const uint32_t *perm, const int64_t *gid, int64_t gid_base,
+                 const uint32_t *cell_start, const int64_t *cell_key, int64_t ncells, int periodic, const double *box_host,
+                 const double *origin_host, const int64_t *ncell_host, double b, uint32_t *parent, int64_t *cell_min,
+                 void *stream);
+int nbk_fof_finalize(const uint32_t *perm, const uint32_t *cell_start, int64_t ncells, const uint32_t *parent,
+                     const int64_t *cell_min, uint32_t *row_root, int64_t *minid, void *stream);
+int nbk_fof_lower(const uint32_t *row_root, int64_t n, const int64_t *new_minid, int64_t ncells, int64_t *root_min,
+                  int64_t *minid, uint64_t *changed, void *stream);
+int nbk_fof_root_counts(const uint32_t *row_root, int64_t n, uint64_t *counts, void *stream);
+int nbk_fof_label_rows(const uint32_t *row_root, int64_t n, const int64_t *cell_label, void *labels, int label_bytes,
+                       void *stream);
+int nbk_fof_segment_reduce(int op, const void *col, int col_dtype, const void *mask, int mask_dtype, const double *thresh,
+                           const double *ref, int periodic, const double *box_host, const uint32_t *order,
+                           const int64_t *chunk_first, const int64_t *chunk_label, int64_t nchunks,
+                           const int64_t *label_chunk, int64_t nlabels, double *partial, double *out, void *stream);
+
 /* elementwise helpers behind RealField/ComplexField `[...] = v`, `*= a`, `+= other`
  * (source/mesh/catalog.py:203,354,396-398; fftpower.py:128).  n counts REAL scalars. */
 int nbk_fill(void *x, int dtype, int64_t n, double value, void *stream);

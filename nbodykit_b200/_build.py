@@ -21,6 +21,7 @@ SOURCES = [
     ("binning.cu", ["--fmad=false"]),
     ("ylm.cu", []),
     ("route.cu", ["--fmad=false"]),
+    ("fof.cu", ["--fmad=false"]),
 ]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ARCH + [ "-O3", "-lineinfo", "-std=c++17",

@@ -262,6 +262,24 @@ class SlabLayout(object):
             out.index_add_(0, sidx, back.to(out.dtype))
         return out
 
+    def gather_back_min(self, values, sidx, out):
+        """`gather_back` combining with the minimum (pmesh `layout.gather(mode=numpy.fmin)`): out[source row] becomes the
+        smaller of itself and every value computed for its copies"""
+        nsend = int(sum(self.sendcounts))
+        back = torch.empty(nsend, dtype=values.dtype, device=values.device)
+        self.comm.all_to_all_single(back, values.contiguous(), list(self.sendcounts), list(self.recvcounts))
+        if nsend:
+            out.scatter_reduce_(0, sidx, back.to(out.dtype), reduce="amin", include_self=True)
+        return out
+
+    def route_rows(self, values, sidx):
+        """per-row values of the local rows to their copies: entry k of the result belongs to the k-th row received by
+        `route` (sidx: the source rows `route(..., want_index=True)` returned)"""
+        send = values.index_select(0, sidx) if sidx.numel() else values[:0]
+        recv = torch.empty((int(sum(self.recvcounts)),) + tuple(values.shape[1:]), dtype=values.dtype, device=values.device)
+        self.comm.all_to_all_single(recv, send.contiguous(), list(self.recvcounts), list(self.sendcounts))
+        return recv
+
     def exchange(self, data):
         t = as_device_tensor(data) if not isinstance(data, torch.Tensor) else data
         P = self.comm.size
