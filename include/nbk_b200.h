@@ -339,6 +339,9 @@ int nbk_resample_unpack(const void *recv, void *dst, int dtype, const int64_t *n
 #define NBK_FOF_RED_SUM 2
 int nbk_fof_cell_keys(const void *pos, int pos_dtype, int64_t n, int periodic, const double *box_host,
                       const double *origin_host, const int64_t *ncell_host, double b, int64_t *keys, void *stream);
+/*   grid_keys   : the keys of cell_keys on a grid of any cell size (no linking length; used by the pair counts). */
+int nbk_fof_grid_keys(const void *pos, int pos_dtype, int64_t n, int periodic, const double *box_host,
+                      const double *origin_host, const int64_t *ncell_host, int64_t *keys, void *stream);
 int64_t nbk_fof_sort_workspace(int64_t n, int key_bytes);
 int nbk_fof_sort(void *keys, void *keys_alt, uint32_t *rows, uint32_t *rows_alt, int64_t n, int key_bytes, int end_bit,
                  void *work, int64_t work_bytes, int *result_in_alt, void *stream);
@@ -364,6 +367,28 @@ int nbk_fof_segment_reduce(int op, const void *col, int col_dtype, const void *m
                            const double *ref, int periodic, const double *box_host, const uint32_t *order,
                            const int64_t *chunk_first, const int64_t *chunk_label, int64_t nchunks,
                            const int64_t *label_chunk, int64_t nlabels, double *partial, double *out, void *stream);
+
+/* Binned pair counts in a simulation box (algorithms/paircount.py: SimulationBoxPairCount; DESIGN.md 4.6).  Positions
+ * are double [n][3] with the line of sight in the last column (periodic: already wrapped), both catalogues key-sorted on
+ * the same grid of ncell_host[d] cells of side box[d] / ncell[d] (nbk_fof_grid_keys / sort / compact / sorted_pos).
+ * Primary chunk k = sorted primary rows [chunk_first[k], chunk_first[k+1]), at most nbk_paircount_chunk_rows() rows of
+ * the one cell chunk_key[k].  Secondaries: spos / sw sorted, cell table scell_start[nscells + 1] / scell_key[nscells].
+ * tol_host[d]: how far a row may lie outside its cell (cells are skipped only when every pair is out of range by more).
+ * mode NBK_PC_1D: bins of s over `edges`; NBK_PC_2D: (s, mu = |dc| / s) over edges x edges2 (mu = 1 in the last bin);
+ * NBK_PC_PROJECTED: (r_p, |dc|) over edges x edges2 for |dc| < pimax.  Bin k of `edges` holds e_k^2 <= x^2 < e_{k+1}^2
+ * (squares taken here in double).  Accumulates (device, zero first) npairs[nbins] (uint64), wsum[nbins] (sum of
+ * pw * sw) and ssum[nbins] (sum of s, or r_p), and *candidates (uint64) += pairs tested.  work: device double scratch
+ * of len(edges) + len(edges2) (1d: + 2) entries.  Histograms above nbk_paircount_smem_bins() bins take global atomics. */
+#define NBK_PC_1D 1
+#define NBK_PC_2D 2
+#define NBK_PC_PROJECTED 3
+int64_t nbk_paircount_chunk_rows(void);
+int64_t nbk_paircount_smem_bins(void);
+int nbk_paircount(int mode, const double *ppos, const double *pw, const int64_t *chunk_first, const int64_t *chunk_key,
+                  int64_t nchunks, const double *spos, const double *sw, const uint32_t *scell_start, const int64_t *scell_key,
+                  int64_t nscells, int periodic, const double *box_host, const int64_t *ncell_host, const double *tol_host,
+                  const double *edges_host, int nedges, const double *edges2_host, int nedges2, double pimax, double *work,
+                  uint64_t *npairs, double *wsum, double *ssum, uint64_t *candidates, void *stream);
 
 /* elementwise helpers behind RealField/ComplexField `[...] = v`, `*= a`, `+= other`
  * (source/mesh/catalog.py:203,354,396-398; fftpower.py:128).  n counts REAL scalars. */

@@ -22,6 +22,7 @@ SOURCES = [
     ("ylm.cu", []),
     ("route.cu", ["--fmad=false"]),
     ("fof.cu", ["--fmad=false"]),
+    ("paircount.cu", ["--fmad=false"]),
 ]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ARCH + [ "-O3", "-lineinfo", "-std=c++17",

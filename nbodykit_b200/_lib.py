@@ -77,6 +77,7 @@ SIGNATURES = {
     "nbk_ylm_mul_complex_acc": ([_vp, _vp, _i, _i, _i, _pi64, _pd, _i, _i64, _i64, _vp], _i),
     "nbk_cross_power": ([_vp, _vp, _vp, _i, _i64, _d, _i, _vp], _i),
     "nbk_fof_cell_keys": ([_vp, _i, _i64, _i, _pd, _pd, _pi64, _d, _vp, _vp], _i),
+    "nbk_fof_grid_keys": ([_vp, _i, _i64, _i, _pd, _pd, _pi64, _vp, _vp], _i),
     "nbk_fof_sorted_pos": ([_vp, _i, _i64, _vp, _i, _pd, _vp, _vp], _i),
     "nbk_fof_compact_workspace": ([_i64], _i64),
     "nbk_fof_sort_workspace": ([_i64, _i], _i64),
@@ -89,6 +90,10 @@ SIGNATURES = {
     "nbk_fof_root_counts": ([_vp, _i64, _vp, _vp], _i),
     "nbk_fof_label_rows": ([_vp, _i64, _vp, _vp, _i, _vp], _i),
     "nbk_fof_segment_reduce": ([_i, _vp, _i, _vp, _i, _vp, _vp, _i, _pd, _vp, _vp, _vp, _i64, _vp, _i64, _vp, _vp, _vp], _i),
+    "nbk_paircount_chunk_rows": ([], _i64),
+    "nbk_paircount_smem_bins": ([], _i64),
+    "nbk_paircount": ([_i, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _i, _pd, _pi64, _pd, _pd, _i, _pd, _i, _d, _vp,
+                       _vp, _vp, _vp, _vp, _vp], _i),
     "nbk_fill": ([_vp, _i, _i64, _d, _vp], _i),
     "nbk_scale": ([_vp, _i, _i64, _d, _vp], _i),
     "nbk_axpy": ([_vp, _vp, _i, _i64, _d, _vp], _i),

@@ -414,9 +414,8 @@ __global__ void __launch_bounds__(256) k_fof_reduce_labels(int op, const double 
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-static int fof_geom(FofGeom &g, int periodic, const double *box, const double *origin, const int64_t *ncell, double b) {
-    NBK_CHECK_ARG(box != nullptr && ncell != nullptr, "fof: box and cell counts are required");
-    NBK_CHECK_ARG(b > 0 && isfinite(b), "fof: linking length must be positive and finite (got %g)", b);
+// the cell grid alone (box, origin, cell counts); b = 0 leaves reach / full / b2 unset (nbk_fof_grid_keys)
+static int fof_grid(FofGeom &g, int periodic, const double *box, const double *origin, const int64_t *ncell, double b) {
     double cells = 1.0;
     for (int d = 0; d < 3; d++) {
         NBK_CHECK_ARG(isfinite(box[d]) && box[d] > 0, "fof: box side %d must be positive and finite (got %g)", d, box[d]);
@@ -428,15 +427,25 @@ static int fof_geom(FofGeom &g, int periodic, const double *box, const double *o
         g.org[d] = periodic ? 0.0 : origin[d];
         g.nc[d] = ncell[d];
         g.inv[d] = (double)ncell[d] / box[d];
-        double cs = box[d] / (double)ncell[d];
-        NBK_CHECK_ARG(3.0 * cs * cs <= b * b, "fof: cells on axis %d are wider than b / sqrt(3)", d);
-        g.reach[d] = (long long)floor(b / cs * (1.0 + 1e-12)) + 1;
-        g.full[d] = periodic && 2 * g.reach[d] + 1 >= g.nc[d];
+        g.reach[d] = 0;
+        g.full[d] = 0;
+        if (b > 0) {
+            double cs = box[d] / (double)ncell[d];
+            NBK_CHECK_ARG(3.0 * cs * cs <= b * b, "fof: cells on axis %d are wider than b / sqrt(3)", d);
+            g.reach[d] = (long long)floor(b / cs * (1.0 + 1e-12)) + 1;
+            g.full[d] = periodic && 2 * g.reach[d] + 1 >= g.nc[d];
+        }
     }
     NBK_CHECK_ARG(cells < 9.2e18, "fof: %g cells do not fit a 63-bit key", cells);
     g.periodic = periodic ? 1 : 0;
     g.b2 = b * b;
     return NBK_OK;
+}
+
+static int fof_geom(FofGeom &g, int periodic, const double *box, const double *origin, const int64_t *ncell, double b) {
+    NBK_CHECK_ARG(box != nullptr && ncell != nullptr, "fof: box and cell counts are required");
+    NBK_CHECK_ARG(b > 0 && isfinite(b), "fof: linking length must be positive and finite (got %g)", b);
+    return fof_grid(g, periodic, box, origin, ncell, b);
 }
 
 #define FOF_CHECK_N(n) NBK_CHECK_ARG((n) >= 0 && (n) < (1ll << 32), "fof: row count %lld out of range", (long long)(n))
@@ -448,6 +457,24 @@ extern "C" int nbk_fof_cell_keys(const void *pos, int pos_dtype, int64_t n, int 
     FOF_CHECK_N(n);
     FofGeom g;
     int rc = fof_geom(g, periodic, box_host, origin_host, ncell_host, b);
+    if (rc) return rc;
+    if (n == 0) return NBK_OK;
+    cudaStream_t s = (cudaStream_t)stream;
+    int grid = nbk_grid_for(n, 256, 8);
+    if (pos_dtype == NBK_F4) k_fof_keys<float><<<grid, 256, 0, s>>>((const float *)pos, n, g, (long long *)keys);
+    else k_fof_keys<double><<<grid, 256, 0, s>>>((const double *)pos, n, g, (long long *)keys);
+    NBK_LAUNCHED();
+    return NBK_OK;
+}
+
+// the keys of nbk_fof_cell_keys on a grid of any cell size (the pair counts choose cells from their largest separation)
+extern "C" int nbk_fof_grid_keys(const void *pos, int pos_dtype, int64_t n, int periodic, const double *box_host,
+                                 const double *origin_host, const int64_t *ncell_host, int64_t *keys, void *stream) {
+    FOF_CHECK_DT(pos_dtype);
+    FOF_CHECK_N(n);
+    NBK_CHECK_ARG(box_host != nullptr && ncell_host != nullptr, "fof: box and cell counts are required");
+    FofGeom g;
+    int rc = fof_grid(g, periodic, box_host, origin_host, ncell_host, 0.0);
     if (rc) return rc;
     if (n == 0) return NBK_OK;
     cudaStream_t s = (cudaStream_t)stream;
