@@ -390,6 +390,25 @@ int nbk_paircount(int mode, const double *ppos, const double *pw, const int64_t 
                   const double *edges_host, int nedges, const double *edges2_host, int nedges2, double pimax, double *work,
                   uint64_t *npairs, double *wsum, double *ssum, uint64_t *candidates, void *stream);
 
+/* Multipoles of the isotropic three-point function in a simulation box (algorithms/threeptcf.py: SimulationBox3PCF;
+ * DESIGN.md 4.7).  Positions, chunks and the secondary cell table as for nbk_paircount (chunks of at most
+ * nbk_threeptcf_chunk_rows() primaries of one cell; no line-of-sight reordering).  Per axis d = x_j - x_p in double
+ * (periodic: d > L/2 -> d - L, d <= -L/2 -> d + L), r = sqrt((dx^2 + dy^2) + dz^2); radial bin k of `edges` (e_0 >= 0,
+ * at most nbk_threeptcf_max_bins() bins) holds e_k < r <= e_{k+1}, r > 0.  poles_host: npoles distinct l in
+ * 0 .. nbk_threeptcf_max_ell(); L = max l.  coef_host: [(L+1)(L+2)/2][L+1] table T with a_lm = sum_k T[lm][k] M_{m,k},
+ * lm = off(m) + l - m, off(m) = m (L + 1) - m (m - 1) / 2, M_{m,k}(b) = sum_{j in b} w_j (ux + i uy)^m uz^k.
+ * Accumulates (device, zero first) zeta[npoles][nb][nb] (b1 <= b2 only) += sum_p w_p sum_m c_m Re[a_lm(b1) a*_lm(b2)]
+ * with c_0 = 1, c_m = 2 (m > 0), npairs[nb] (uint64, ordered (p, j) pairs per bin) and *candidates += pairs tested.
+ * work: device double scratch of nedges + (L+1)^2 (L+2) / 2 entries. */
+int64_t nbk_threeptcf_chunk_rows(void);
+int nbk_threeptcf_max_ell(void);
+int nbk_threeptcf_max_bins(void);
+int nbk_threeptcf(const double *ppos, const double *pw, const int64_t *chunk_first, const int64_t *chunk_key, int64_t nchunks,
+                  const double *spos, const double *sw, const uint32_t *scell_start, const int64_t *scell_key, int64_t nscells,
+                  int periodic, const double *box_host, const int64_t *ncell_host, const double *tol_host, const double *edges_host,
+                  int nedges, const int *poles_host, int npoles, const double *coef_host, double *work, double *zeta,
+                  uint64_t *npairs, uint64_t *candidates, void *stream);
+
 /* elementwise helpers behind RealField/ComplexField `[...] = v`, `*= a`, `+= other`
  * (source/mesh/catalog.py:203,354,396-398; fftpower.py:128).  n counts REAL scalars. */
 int nbk_fill(void *x, int dtype, int64_t n, double value, void *stream);

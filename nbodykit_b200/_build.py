@@ -23,6 +23,7 @@ SOURCES = [
     ("route.cu", ["--fmad=false"]),
     ("fof.cu", ["--fmad=false"]),
     ("paircount.cu", ["--fmad=false"]),
+    ("threeptcf.cu", ["--fmad=false"]),
 ]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ARCH + [ "-O3", "-lineinfo", "-std=c++17",
@@ -38,7 +39,8 @@ def _nvcc():
 
 def _stamp(path, flags):
     h = hashlib.sha1()
-    for dep in [path, os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "ylm_table.inc"),
+    for dep in [path, os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "pc_cells.cuh"),
+                os.path.join(CSRC, "ylm_table.inc"),
                 os.path.join(HERE, "..", "include", "nbk_b200.h")]:
         with open(dep, "rb") as f:
             h.update(f.read())

@@ -94,6 +94,11 @@ SIGNATURES = {
     "nbk_paircount_smem_bins": ([], _i64),
     "nbk_paircount": ([_i, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _i, _pd, _pi64, _pd, _pd, _i, _pd, _i, _d, _vp,
                        _vp, _vp, _vp, _vp, _vp], _i),
+    "nbk_threeptcf_chunk_rows": ([], _i64),
+    "nbk_threeptcf_max_ell": ([], _i),
+    "nbk_threeptcf_max_bins": ([], _i),
+    "nbk_threeptcf": ([_vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _i, _pd, _pi64, _pd, _pd, _i, _pi, _i, _pd, _vp,
+                       _vp, _vp, _vp, _vp], _i),
     "nbk_fill": ([_vp, _i, _i64, _d, _vp], _i),
     "nbk_scale": ([_vp, _i, _i64, _d, _vp], _i),
     "nbk_axpy": ([_vp, _vp, _i, _i64, _d, _vp], _i),

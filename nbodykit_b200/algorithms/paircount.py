@@ -150,6 +150,50 @@ def count_pairs(mode, pos1, w1, pos2, w2, edges, periodic, box, los=2, Nmu=None,
     return npairs, wsum, ssum, int(cand.item())
 
 
+def slab_route(comm, pos1, w1, pos2, w2, periodic, box, smax):
+    """(primaries, their weights, secondaries, their weights) of this rank's x slab: every row of pos1 on the rank
+    whose slab holds it, and every row of pos2 on its own rank plus copies on each remote slab within smax of it"""
+    P = comm.size
+    if periodic:
+        rbox = box
+        r1, r2 = pos1, pos2
+    else:
+        def bounds(p):
+            if p.shape[0] == 0:
+                return numpy.inf, -numpy.inf
+            x = p[:, 0]
+            return float(x.min().item()), float(x.max().item())
+        b = [bounds(pos1), bounds(pos2)]
+        lo = min(min(v[0] for v in comm.allgather(bb)) for bb in b)
+        hi = max(max(v[1] for v in comm.allgather(bb)) for bb in b)
+        lo = lo if numpy.isfinite(lo) else 0.0
+        rbox = numpy.array([hi - lo if hi > lo else 1.0, 1.0, 1.0])
+        # slabs of [lo, hi] in double, so that the shift by lo cannot move a row across a slab edge
+        r1 = pos1.to(torch.float64, copy=True)
+        r1[:, 0] -= lo
+        r2 = r1 if pos2 is pos1 else pos2.to(torch.float64, copy=True)
+        if pos2 is not pos1:
+            r2[:, 0] -= lo
+    pm = ParticleMesh(BoxSize=rbox, Nmesh=[P, P, P], dtype='f8', comm=comm)
+    # primaries: every row belongs to the one slab holding floor(x P / Lx); rows listed by the zero-reach routing
+    # are remote, all others stay
+    lay1 = pm._decompose_device(r1, 0.0)
+    keep = torch.ones(int(pos1.shape[0]), dtype=torch.bool, device=pos1.device)
+    if lay1.ghosts.numel():
+        keep[(lay1.ghosts & 0xffffffff)] = False
+    rp1, rw1 = lay1.route(pos1, mass=w1)
+    prim = torch.cat([pos1[keep], rp1])
+    pw = torch.cat([w1[keep], rw1])
+    # secondaries: copies of the rows within s_max of a remote slab, widened a little so that the rounding of
+    # x P / Lx can never drop a needed copy; a reach of P + 1 slabs already reaches every slab
+    smoothing = min(smax * P / float(rbox[0]) * (1 + 1e-6) + 1e-9, P + 1.0)
+    lay2 = pm._decompose_device(r2, smoothing)
+    rp2, rw2 = lay2.route(pos2, mass=w2)
+    sec = torch.cat([pos2, rp2])
+    sw = torch.cat([w2, rw2])
+    return prim.contiguous(), pw.contiguous(), sec.contiguous(), sw.contiguous()
+
+
 def _verify_sources(first, second, BoxSize, columns):
     """the box of the count from the sources' attrs and the `BoxSize` keyword; every source must hold `columns`"""
     if second is None:
@@ -351,46 +395,7 @@ class SimulationBoxPairCount(object):
 
     def _route(self, pos1, w1, pos2, w2, periodic, box, smax):
         """(primaries, their weights, secondaries, their weights) of this rank's x slab"""
-        comm = self.comm
-        P = comm.size
-        if periodic:
-            rbox = box
-            r1, r2 = pos1, pos2
-        else:
-            def bounds(p):
-                if p.shape[0] == 0:
-                    return numpy.inf, -numpy.inf
-                x = p[:, 0]
-                return float(x.min().item()), float(x.max().item())
-            b = [bounds(pos1), bounds(pos2)]
-            lo = min(min(v[0] for v in comm.allgather(bb)) for bb in b)
-            hi = max(max(v[1] for v in comm.allgather(bb)) for bb in b)
-            lo = lo if numpy.isfinite(lo) else 0.0
-            rbox = numpy.array([hi - lo if hi > lo else 1.0, 1.0, 1.0])
-            # slabs of [lo, hi] in double, so that the shift by lo cannot move a row across a slab edge
-            r1 = pos1.to(torch.float64, copy=True)
-            r1[:, 0] -= lo
-            r2 = r1 if pos2 is pos1 else pos2.to(torch.float64, copy=True)
-            if pos2 is not pos1:
-                r2[:, 0] -= lo
-        pm = ParticleMesh(BoxSize=rbox, Nmesh=[P, P, P], dtype='f8', comm=comm)
-        # primaries: every row belongs to the one slab holding floor(x P / Lx); rows listed by the zero-reach routing
-        # are remote, all others stay
-        lay1 = pm._decompose_device(r1, 0.0)
-        keep = torch.ones(int(pos1.shape[0]), dtype=torch.bool, device=pos1.device)
-        if lay1.ghosts.numel():
-            keep[(lay1.ghosts & 0xffffffff)] = False
-        rp1, rw1 = lay1.route(pos1, mass=w1)
-        prim = torch.cat([pos1[keep], rp1])
-        pw = torch.cat([w1[keep], rw1])
-        # secondaries: copies of the rows within s_max of a remote slab, widened a little so that the rounding of
-        # x P / Lx can never drop a needed copy; a reach of P + 1 slabs already reaches every slab
-        smoothing = min(smax * P / float(rbox[0]) * (1 + 1e-6) + 1e-9, P + 1.0)
-        lay2 = pm._decompose_device(r2, smoothing)
-        rp2, rw2 = lay2.route(pos2, mass=w2)
-        sec = torch.cat([pos2, rp2])
-        sw = torch.cat([w2, rw2])
-        return prim.contiguous(), pw.contiguous(), sec.contiguous(), sw.contiguous()
+        return slab_route(self.comm, pos1, w1, pos2, w2, periodic, box, smax)
 
     def _reduce(self, npairs, wsum, ssum, cand):
         """host arrays of the histograms summed over ranks, in one all-reduce (counts as two exact 32-bit halves)"""
