@@ -1,6 +1,10 @@
 // cuFFT-free 3-D real<->complex FFT (RealField.r2c / ComplexField.c2r: base/mesh.py:228,237;
 // source/mesh/catalog.py:341-351).  Forward is normalised by 1/prod(N), backward is not
 // (source/mesh/array.py:36-37, fftpower.py:126-128).
+// c2r contract: for ANY half spectrum X [Nx][Ny][Nz/2+1] (no symmetry assumed) the result is irfftn(X, s=N) * prod(N),
+// the rule of numpy / scipy irfftn and of FFTW's c2r: complex inverses along x and y, then a real inverse along z that
+// drops the imaginary parts of the kz = 0 entry and, for even Nz, of the kz = Nz/2 entry.  Every inverse z pass (power
+// of two, mixed radix, Bluestein; even and odd Nz) makes those entries real before it uses them.
 //
 // Structure: three line passes, each one read + one write of the field (HBM-bound):
 //   z pass  : rows are contiguous; real row of Nz -> packed complex FFT of Nz/2 -> Nz/2+1 modes
@@ -1138,6 +1142,7 @@ k_fft_z_c2r(const typename C2<T>::type *__restrict__ cplx, T *__restrict__ real,
             if (b < bvalid) {
                 C xk = src[(int64_t)b * Nzc + k];
                 C xm = cconj(src[(int64_t)b * Nzc + (M - k)]);
+                if (k == 0) { xk.y = 0; xm.y = 0; }     // the k = 0 and k = Nz/2 modes of a real row are real
                 C e = cadd(xk, xm), d = csub(xk, xm);
                 C o = cmul(cconj(twN[k]), d);
                 // Z = (e + i o)/2 ; the factor 2 of the unnormalised inverse cancels the 1/2
@@ -2285,8 +2290,9 @@ k_fft_z_mixed(const void *in, void *out, const typename C2<T>::type *__restrict_
                 const int b = w / L, k = w - b * L;
                 C z = C{0, 0};
                 if (b < nrows) {
-                    const C xk = src[(int64_t)b * Nzc + k];
-                    const C xm = cconj(src[(int64_t)b * Nzc + (L - k)]);
+                    C xk = src[(int64_t)b * Nzc + k];
+                    C xm = cconj(src[(int64_t)b * Nzc + (L - k)]);
+                    if (k == 0) { xk.y = 0; xm.y = 0; }     // the k = 0 and k = Nz/2 modes of a real row are real
                     const C e = cadd(xk, xm), d = csub(xk, xm);
                     const C o = cmul(cconj(tw[k]), d);
                     z = C{e.x - o.y, e.y + o.x};
@@ -2715,8 +2721,9 @@ k_fft_z_bluestein(const void *in, void *out, const typename C2<T>::type *__restr
                 const int b = w / L, k = w - b * L;
                 C z = C{0, 0};
                 if (b < nrows) {
-                    const C xk = src[(int64_t)b * Nzc + k];
-                    const C xm = cconj(src[(int64_t)b * Nzc + (L - k)]);
+                    C xk = src[(int64_t)b * Nzc + k];
+                    C xm = cconj(src[(int64_t)b * Nzc + (L - k)]);
+                    if (k == 0) { xk.y = 0; xm.y = 0; }     // the k = 0 and k = Nz/2 modes of a real row are real
                     const C e = cadd(xk, xm), d = csub(xk, xm);
                     const C o = cmul(cconj(twz[k]), d);
                     z = C{e.x - o.y, e.y + o.x};

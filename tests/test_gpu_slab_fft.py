@@ -9,7 +9,8 @@ driven kernel by kernel:
     buffer viewed as [x_n][Ny][Nzc], y + z c2r;
   * all-to-all route: pack, a block swap done here (block q of rank r's receive buffer is block r of rank q's send
     buffer), unpack, in-place line pass.
-A non-Hermitian spectrum has no NumPy c2r: there both routes must agree with the single-GPU nbk_c2r of the same input.
+A spectrum with no symmetry has a NumPy c2r as well, irfftn (complex inverses along x and y, a real inverse along z that
+drops the imaginary parts of the kz = 0 and kz = Nz/2 entries): both routes and the single-GPU nbk_c2r must equal it.
 
 The peer route needs symmetric memory shared between processes, which one process on one GPU does not have, so these
 tests check the kernels with their own copy of the arguments of pm.py's peer branch: an argument error in that branch
@@ -239,8 +240,8 @@ def test_slab_r2c_c2r(cuda, case, dtype, route):
 @pytest.mark.parametrize("case", SLAB_CASES, ids=_ids)
 @pytest.mark.parametrize("dtype", ["f8", "f4"])
 def test_slab_c2r_general_input_equals_one_gpu(cuda, case, dtype):
-    """a spectrum with no symmetry (complex kz = 0 and Nyquist planes included): both distributed inverses run the x,
-    y, z passes of the single-GPU nbk_c2r on the same input, so they agree with it to rounding"""
+    """a spectrum with no symmetry (complex kz = 0 and Nyquist planes included): the single-GPU nbk_c2r equals irfftn
+    N^3 of it, and both distributed inverses, which run the same x, y, z passes, agree with nbk_c2r to rounding"""
     import torch
     _l = _lib()
     Nx, Ny, Nz, P = case
@@ -256,11 +257,14 @@ def test_slab_c2r_general_input_equals_one_gpu(cuda, case, dtype):
     want = _host(one).astype("f8")
     np.testing.assert_array_equal(_host(full), c)          # nbk_c2r with `work` keeps its input
     rms = np.sqrt((want ** 2).mean())
+    ref = np.fft.irfftn(c.astype("c16"), s=N, axes=(0, 1, 2)) * n
+    assert np.abs(want - ref).max() <= TOL[dtype] * rms * np.log2(n) * 10, "nbk_c2r vs irfftn"
     for route, (_, inv) in sorted(ROUTES.items()):
         specs = _split_y(c, P)
         got = _join_x(inv(specs, N, P, dtype))
         err = np.abs(got - want).max()
         assert err <= TOL[dtype] * rms * np.log2(n), "%s: %g vs rms %g" % (route, err, rms)
+        assert np.abs(got - ref).max() <= TOL[dtype] * rms * np.log2(n) * 10, "%s vs irfftn" % route
         if route == "peer":                                 # the peer inverse only reads its input
             np.testing.assert_array_equal(_join_y(specs), c)
 
