@@ -28,6 +28,9 @@ from ..fftpower import _find_unique_edges, project_to_basis_device
 from .catalog import FKPCatalog
 from .catalogmesh import FKPCatalogMesh
 
+# largest l of the real spherical harmonics the device evaluates (NBK_YLM_LMAX of csrc/ylm_table.inc, tools/gen_ylm.py)
+YLM_LMAX = 8
+
 
 class ConvolvedFFTPower(object):
     """
@@ -47,6 +50,11 @@ class ConvolvedFFTPower(object):
             raise ValueError("use_fkp_weights and P0_FKP are deprecated. Assign a FKPWeight column to "
                              "source['randoms']['FKPWeight'] and source['data']['FKPWeight'] with the help of "
                              "the FKPWeightFromNbar(nbar) function")
+        # Y_lm exists on the device up to the generated table's l (csrc/ylm_table.inc): refuse larger l before any
+        # paint or FFT runs
+        if any(int(ell) > YLM_LMAX for ell in numpy.atleast_1d(poles)):
+            raise ValueError("ConvolvedFFTPower computes multipoles l <= %d (the Y_lm table limit); got poles=%s"
+                             % (YLM_LMAX, list(numpy.atleast_1d(poles))))
         first = _cast_mesh(first, Nmesh=Nmesh)
         if second is not None:
             second = _cast_mesh(second, Nmesh=Nmesh)

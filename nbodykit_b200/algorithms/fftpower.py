@@ -340,12 +340,20 @@ def project_to_basis_device(y3d, edges, los=[0, 0, 1], poles=[], coord_dtype="f4
     nb = (Nx + 2) * (Nmu + 2)
 
     dev = y3d.value.device
-    # one packed accumulator: [nsum(i64 bits) | xsum | musum | ysum(Nell*nb*2)] so a single all-reduce suffices
+    # one launch bins at most 8 multipoles (NBK_MAX_ELL), the first of them l = 0: any number of poles is binned in
+    # groups, _poles[:8] and then [0] + the next 7, each group into its own rows of ysum.  The l = 0 row of every
+    # further group repeats the first group's and is dropped.
+    groups = [_poles[:8]] + [[0] + _poles[i:i + 7] for i in range(8, Nell, 7)]
+    nrow = sum(len(grp) for grp in groups)
+    # one packed accumulator: [xsum | musum | ysum(nrow*nb*2)] (and nsum) so a single all-reduce suffices
     nsum = torch.zeros(nb, dtype=torch.int64, device=dev)
-    facc = torch.zeros(nb * (2 + 2 * Nell), dtype=torch.float64, device=dev)
+    facc = torch.zeros(nb * (2 + 2 * nrow), dtype=torch.float64, device=dev)
     xsum = facc[:nb]
     musum = facc[nb:2 * nb]
-    ysum = facc[2 * nb:]
+    # the counts and k sums of the further groups repeat the first group's: they go to a scratch pair that is not reduced
+    if len(groups) > 1:
+        spare_n = torch.zeros(nb, dtype=torch.int64, device=dev)
+        spare_x = torch.zeros(nb, dtype=torch.float64, device=dev)
     tr, start, count = (0, pm.x_start, pm.x_n) if is_real else y3d._slab()
     los_f = [float(v) for v in los]
     herm = 0 if (is_real or not y3d.compressed) else (2 if antihermitian else 1)
@@ -354,13 +362,20 @@ def project_to_basis_device(y3d, edges, los=[0, 0, 1], poles=[], coord_dtype="f4
     with stage("power_bin"):
         fn = lib().nbk_power_bin if mirror is None else lib().nbk_power_bin2
         extra = () if mirror is None else (_ptr(mirror.value),)
-        check(fn(
-            _ptr(y3d.value), _ptr(second.value) if second is not None else None, *extra, _CODE[pm.typestr],
-            1 if is_p3d else 0, float(volume), 1 if clear_zero else 0, pm._nmesh_c, pm._box_c, tr, start, count,
-            _los_coord_mode(los, coord_dtype), _lib.darr(x2edges), Nx, _lib.darr(muedges), Nmu, _lib.darr(los_f),
-            _lib.i32arr(_poles), Nell, herm, _lib.COMP.get(compensation[0], 0),
-            _lib.COMP.get(compensation[1], 0), 1 if is_real else 0, coord_unit,
-            _ptr(nsum), _ptr(xsum), _ptr(musum) if need_mu else None, _ptr(ysum), _stream()), "nbk_power_bin")
+        row, keep = 0, []
+        for i, grp in enumerate(groups):
+            first = i == 0
+            check(fn(
+                _ptr(y3d.value), _ptr(second.value) if second is not None else None, *extra, _CODE[pm.typestr],
+                1 if is_p3d else 0, float(volume), 1 if clear_zero else 0, pm._nmesh_c, pm._box_c, tr, start, count,
+                _los_coord_mode(los, coord_dtype), _lib.darr(x2edges), Nx, _lib.darr(muedges), Nmu, _lib.darr(los_f),
+                _lib.i32arr(grp), len(grp), herm, _lib.COMP.get(compensation[0], 0),
+                _lib.COMP.get(compensation[1], 0), 1 if is_real else 0, coord_unit,
+                _ptr(nsum if first else spare_n), _ptr(xsum if first else spare_x),
+                _ptr(musum) if (need_mu and first) else None, _ptr(facc[(2 + 2 * row) * nb:]), _stream()),
+                "nbk_power_bin")
+            keep += range(row if first else row + 1, row + len(grp))
+            row += len(grp)
     with stage("H:bin_reduce"):
         if comm.size > 1:
             comm.allreduce_tensor(nsum)
@@ -369,7 +384,7 @@ def project_to_basis_device(y3d, edges, los=[0, 0, 1], poles=[], coord_dtype="f4
         f = facc.cpu().numpy()
     xsum = f[:nb].reshape(Nx + 2, Nmu + 2)
     musum = f[nb:2 * nb].reshape(Nx + 2, Nmu + 2)
-    ysum = f[2 * nb:].reshape(Nell, Nx + 2, Nmu + 2, 2)
+    ysum = f[2 * nb:].reshape(nrow, Nx + 2, Nmu + 2, 2)[keep]
     ysum = ysum[..., 0] + 1j * ysum[..., 1]
 
     # fold the mu == 1 overflow bin, form the means (fftpower.py:674-701)

@@ -231,10 +231,23 @@ def _legendre_coeffs(ell):
     return np.asarray(legendre(ell).coeffs, dtype="f8")
 
 
-def project_sums(y3d, x3d, edges, los=(0, 0, 1), poles=(), hermitian_symmetric=True, planes=None):
+def _legendre_horner(ell, mu):
+    """numpy.poly1d.__call__ of scipy.special.legendre(ell) = polyval: Horner with f8 coefficients on mu.  The
+    reference calls legendre(ell)(mu), which scipy 1.18's orthopoly1d routes to eval_legendre; a plain poly1d takes
+    this Horner form, whose cancellation error grows past 1e-10 at ell = 16 and past 1 at ell = 40"""
+    leg = np.zeros_like(mu, dtype="f8")
+    for pv in _legendre_coeffs(ell):
+        leg = leg * mu + pv
+    return leg
+
+
+def project_sums(y3d, x3d, edges, los=(0, 0, 1), poles=(), hermitian_symmetric=True, planes=None, legendre=None):
     """the raw per-bin sums of `project_to_basis` over the x-planes `planes` (default: all) -- what one MPI rank
     of the reference accumulates before the allreduce (fftpower.py:605-672).  Returns (xsum, musum, ysum, Nsum)
-    shaped (Nx+2, Nmu+2) [ysum: (Nell, Nx+2, Nmu+2)]."""
+    shaped (Nx+2, Nmu+2) [ysum: (Nell, Nx+2, Nmu+2)].
+    `legendre(ell, mu)` gives the weights (default: Horner on the coefficients of scipy.special.legendre, see
+    _legendre_horner; pass scipy.special.eval_legendre above ell ~ 8, where the Horner form loses digits)."""
+    legendre = _legendre_horner if legendre is None else legendre
     xedges, muedges = edges
     x2edges = np.asarray(xedges) ** 2
     Nx = len(xedges) - 1
@@ -280,10 +293,8 @@ def project_sums(y3d, x3d, edges, los=(0, 0, 1), poles=(), hermitian_symmetric=T
                             minlength=nbins).astype("i8")
         yplane = y3d[islab]
         for iell, ell in enumerate(_poles):
-            # numpy.poly1d.__call__ = polyval: Horner with f8 coefficients on mu
-            leg = np.zeros_like(mu, dtype="f8")
-            for pv in _legendre_coeffs(ell):
-                leg = leg * mu + pv
+            # (a float32 mu widens exactly, as the kernel widens it)
+            leg = np.asarray(legendre(ell, mu.astype("f8")), dtype="f8")
             wy = (leg * yplane).astype(np.complex128)
             if hermitian_symmetric:
                 if ell % 2:
@@ -304,16 +315,17 @@ def project_sums(y3d, x3d, edges, los=(0, 0, 1), poles=(), hermitian_symmetric=T
     return xsum, musum, ysum, Nsum
 
 
-def project_to_basis(y3d, x3d, edges, los=(0, 0, 1), poles=(), hermitian_symmetric=True):
+def project_to_basis(y3d, x3d, edges, los=(0, 0, 1), poles=(), hermitian_symmetric=True, legendre=None):
     """y3d: ndarray (N0,N1,N2c); x3d: 3 broadcastable coordinate arrays (their dtype is part of the
     contract).  Returns exactly what the reference returns:
-    (xmean_2d, mumean_2d, y2d, N_2d), (xmean_1d, poles, N_1d) | None"""
+    (xmean_2d, mumean_2d, y2d, N_2d), (xmean_1d, poles, N_1d) | None
+    (`legendre`: see project_sums)"""
     poles = list(poles)
     _poles = [0] + sorted(poles) if 0 not in poles else sorted(poles)
     if any(ell < 0 for ell in _poles):
         raise ValueError("in `project_to_basis`, multipole numbers must be non-negative integers")
     ell_idx = [_poles.index(l) for l in poles]
-    xsum, musum, ysum, Nsum = project_sums(y3d, x3d, edges, los, poles, hermitian_symmetric)
+    xsum, musum, ysum, Nsum = project_sums(y3d, x3d, edges, los, poles, hermitian_symmetric, legendre=legendre)
     return finish_projection(xsum, musum, ysum, Nsum, len(poles) > 0, ell_idx)
 
 

@@ -148,7 +148,8 @@ if __name__ == "__main__":
 
 def golden_ylm():
     """values of the REFERENCE's get_real_Ylm (algorithms/convpower/fkp.py:12-73, executed from its source with
-    sympy.lambdify's 'numexpr' backend swapped for 'numpy') on seeded unit vectors and at the origin"""
+    sympy.lambdify's 'numexpr' backend swapped for 'numpy') on seeded unit vectors and at the origin, for every
+    (l, m) of the device table (l <= 8)"""
     import ast
     import sympy
     src = open(os.path.join(refload.REF, "nbodykit/algorithms/convpower/fkp.py")).read()
@@ -164,7 +165,7 @@ def golden_ylm():
         v = rng.standard_normal((64, 3))
         v /= np.sqrt((v ** 2).sum(axis=1))[:, None]
         out = {"vec": v}
-        for l in range(0, 5):
+        for l in range(0, 9):
             for m in range(-l, l + 1):
                 f = ns_["get_real_Ylm"](l, m)
                 val = np.broadcast_to(np.asarray(f(v[:, 0], v[:, 1], v[:, 2]), dtype="f8"), (64,))

@@ -316,7 +316,7 @@ def _fold_mu1(s):
 
 
 @pytest.mark.parametrize("N", [(32, 32, 32), (48, 36, 16), (44, 52, 37), (45, 21, 35)])
-@pytest.mark.parametrize("ell", [1, 2])
+@pytest.mark.parametrize("ell", [1, 2, 3, 5, 8])
 def test_mirror_accumulator(cuda, N, ell):
     """A_l = sum_m c_m Y_lm(khat) and its mirror from nbk_ylm_mul_complex_acc2, binned by nbk_power_bin2 on the
     compressed spectrum (P = 1 and transposed virtual ranks), against the full-z hermitian = 0 binning of the completed
