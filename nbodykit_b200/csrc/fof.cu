@@ -45,11 +45,16 @@ static __device__ __forceinline__ T np_mod(T x, T L) {
     return r;
 }
 
+// Every row must lie inside its cell on every axis (up to rounding), because FOF links every pair of one cell unseen.
+// A periodic row at q >= nc sits at or above the period L: an f4 row wrapped onto L_f4 > L, or an f8 row that `x % L`
+// rounded up to L.  Its minimum image is L_f4 - L (or 0) above 0, so it belongs to cell 0; clamping it into cell
+// nc - 1 would put it up to cs + (L_f4 - L) from that cell's lower corner.
 template <typename T>
 static __device__ __forceinline__ long long cell_of(T p, int d, const FofGeom &g) {
     double q = g.periodic ? (double)p * g.inv[d] : ((double)p - g.org[d]) * g.inv[d];
     long long c = (long long)floor(q);
-    return c < 0 ? 0 : (c >= g.nc[d] ? g.nc[d] - 1 : c);
+    if (c >= g.nc[d]) return g.periodic ? 0 : g.nc[d] - 1;
+    return c < 0 ? 0 : c;
 }
 
 template <typename T>

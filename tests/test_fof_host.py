@@ -85,6 +85,26 @@ def test_features_and_halos_errors_without_running(monkeypatch):
         fof.to_halos(1e12, None, 0.5)
 
 
+def test_cells_per_axis_cap():
+    """2^21 cells of side b / sqrt(3) on an axis are accepted, 2^21 + 1 are not, nor 2^21 on all three axes (a 63-bit
+    key); one cell at least, and the ceil boundary a relative 1e-11 either side"""
+    from nbodykit_b200.algorithms.fof import _cells
+    b = 1.
+    per_cell = b / (np.sqrt(3) * (1 + 1e-9))
+    assert _cells([((1 << 21) - 0.5) * per_cell, 1., 1.], b) == [1 << 21, 2, 2]
+    assert _cells([1., 1., ((1 << 21) - 0.5) * per_cell], b) == [2, 2, 1 << 21]
+    with pytest.raises(ValueError, match="63-bit"):
+        _cells([((1 << 21) + 0.5) * per_cell, 1., 1.], b)
+    with pytest.raises(ValueError, match="63-bit"):
+        _cells([((1 << 21) - 0.5) * per_cell] * 3, b)
+    assert _cells([((1 << 20) + 0.5) * per_cell] * 3, b) == [(1 << 20) + 1] * 3
+    assert _cells([1e-300, 1e-3, 0.5], b) == [1, 1, 1]
+    L, n = 20., 13
+    b0 = L * np.sqrt(3) * (1 + 1e-9) / n
+    assert _cells([L] * 3, b0 * (1 - 1e-11)) == [n + 1] * 3
+    assert _cells([L] * 3, b0 * (1 + 1e-11)) == [n] * 3
+
+
 def test_fof_is_exported():
     import nbodykit_b200.algorithms as alg
     import nbodykit_b200.lab as lab
