@@ -368,20 +368,30 @@ int nbk_fof_segment_reduce(int op, const void *col, int col_dtype, const void *m
                            const int64_t *chunk_first, const int64_t *chunk_label, int64_t nchunks,
                            const int64_t *label_chunk, int64_t nlabels, double *partial, double *out, void *stream);
 
-/* Binned pair counts in a simulation box (algorithms/paircount.py: SimulationBoxPairCount; DESIGN.md 4.6).  Positions
- * are double [n][3] with the line of sight in the last column (periodic: already wrapped), both catalogues key-sorted on
- * the same grid of ncell_host[d] cells of side box[d] / ncell[d] (nbk_fof_grid_keys / sort / compact / sorted_pos).
+/* Binned pair counts in a simulation box or a survey (algorithms/paircount.py: SimulationBoxPairCount,
+ * algorithms/surveypaircount.py: SurveyDataPairCount; DESIGN.md 4.6, 4.8).  Positions are double [n][3] with the line
+ * of sight in the last column (periodic: already wrapped), both catalogues key-sorted on the same grid of
+ * ncell_host[d] cells of side box[d] / ncell[d] (nbk_fof_grid_keys / sort / compact / sorted_pos).
  * Primary chunk k = sorted primary rows [chunk_first[k], chunk_first[k+1]), at most nbk_paircount_chunk_rows() rows of
  * the one cell chunk_key[k].  Secondaries: spos / sw sorted, cell table scell_start[nscells + 1] / scell_key[nscells].
  * tol_host[d]: how far a row may lie outside its cell (cells are skipped only when every pair is out of range by more).
  * mode NBK_PC_1D: bins of s over `edges`; NBK_PC_2D: (s, mu = |dc| / s) over edges x edges2 (mu = 1 in the last bin);
  * NBK_PC_PROJECTED: (r_p, |dc|) over edges x edges2 for |dc| < pimax.  Bin k of `edges` holds e_k^2 <= x^2 < e_{k+1}^2
- * (squares taken here in double).  Accumulates (device, zero first) npairs[nbins] (uint64), wsum[nbins] (sum of
- * pw * sw) and ssum[nbins] (sum of s, or r_p), and *candidates (uint64) += pairs tested.  work: device double scratch
- * of len(edges) + len(edges2) (1d: + 2) entries.  Histograms above nbk_paircount_smem_bins() bins take global atomics. */
+ * (squares taken here in double).  The survey modes (periodic must be 0) take the observer at the origin and the
+ * pair's midpoint as its line of sight: s = x2 - x1, l = x1 + x2 per axis, l^2 = (lx^2 + ly^2) + lz^2,
+ * sl = (sx lx + sy ly) + sz lz.  NBK_PC_SURVEY_2D: (s, mu = |sl| / (s sqrt(l^2)), 0 when l^2 = 0) as NBK_PC_2D;
+ * NBK_PC_SURVEY_PROJECTED: pi = |sl| / sqrt(l^2) (0 when l^2 = 0), r_p^2 = max(s^2 - pi^2, 0), (r_p, pi) as
+ * NBK_PC_PROJECTED for pi < pimax; NBK_PC_ANGULAR: unit vectors, `edges` are chords 2 sin(theta / 2), bins of the chord
+ * as NBK_PC_1D, summing theta = 2 asin(chord / 2) in degrees.  Accumulates (device, zero first) npairs[nbins]
+ * (uint64), wsum[nbins] (sum of pw * sw) and ssum[nbins] (sum of s, r_p or theta), and *candidates (uint64) += pairs
+ * tested.  work: device double scratch of len(edges) + len(edges2) (1d / angular: + 2) entries.  Histograms above
+ * nbk_paircount_smem_bins() bins take global atomics. */
 #define NBK_PC_1D 1
 #define NBK_PC_2D 2
 #define NBK_PC_PROJECTED 3
+#define NBK_PC_SURVEY_2D 4
+#define NBK_PC_SURVEY_PROJECTED 5
+#define NBK_PC_ANGULAR 6
 int64_t nbk_paircount_chunk_rows(void);
 int64_t nbk_paircount_smem_bins(void);
 int nbk_paircount(int mode, const double *ppos, const double *pw, const int64_t *chunk_first, const int64_t *chunk_key,

@@ -3,10 +3,12 @@ from .fftcorr import FFTCorr
 from .fftrecon import FFTRecon
 from .fof import FOF
 from .paircount import SimulationBoxPairCount, SimulationBox2PCF
-from .threeptcf import SimulationBox3PCF
+from .threeptcf import SimulationBox3PCF, SurveyData3PCF
+from .surveypaircount import SurveyDataPairCount, SurveyData2PCF
 from .convpower import ConvolvedFFTPower, FKPCatalog, FKPWeightFromNbar, FKPCatalogMesh
 
 FKPPower = ConvolvedFFTPower
 
-__all__ = ['FOF', 'SimulationBoxPairCount', 'SimulationBox2PCF', 'SimulationBox3PCF', 'FFTCorr', 'FFTRecon', 'FFTPower', 'ProjectedFFTPower', 'FFTBase', 'project_to_basis', 'ConvolvedFFTPower', 'FKPPower', 'FKPCatalog',
+__all__ = ['FOF', 'SimulationBoxPairCount', 'SimulationBox2PCF', 'SimulationBox3PCF', 'SurveyDataPairCount',
+           'SurveyData2PCF', 'SurveyData3PCF', 'FFTCorr', 'FFTRecon', 'FFTPower', 'ProjectedFFTPower', 'FFTBase', 'project_to_basis', 'ConvolvedFFTPower', 'FKPPower', 'FKPCatalog',
            'FKPWeightFromNbar', 'FKPCatalogMesh']

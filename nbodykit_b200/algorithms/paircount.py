@@ -27,6 +27,8 @@ from ..pmesh.pm import ParticleMesh, _ptr, _stream
 from .fof import _code, _column, _sort_rows
 
 _MODES = {'1d': 1, '2d': 2, 'projected': 3}
+# the kernel modes of survey pairs, whose line of sight is the pair's midpoint as seen from the origin (DESIGN.md 4.8)
+_SURVEY_KERNEL_MODES = {'1d': 1, '2d': 4, 'projected': 5, 'angular': 6}
 # cells per s_max along each axis: the neighbour stencil is 5 cells wide, and the corner columns and cells whose
 # nearest point is beyond s_max are skipped (DESIGN.md 4.6)
 _CELLS_PER_SMAX = 2
@@ -104,9 +106,10 @@ class _Cells(object):
         return first.contiguous(), self.cell_key[cell].contiguous(), nchunks
 
 
-def count_pairs(mode, pos1, w1, pos2, w2, edges, periodic, box, los=2, Nmu=None, pimax=None):
+def count_pairs(mode, pos1, w1, pos2, w2, edges, periodic, box, los=2, Nmu=None, pimax=None, survey=False):
     """binned ordered pairs of the rows of pos1 (primaries) against those of pos2 on this device, per the contract of
-    DESIGN.md 4.6.  pos: (n, 3) float32 / float64 device tensors in box coordinates; w: float64 (n,).  Returns device
+    DESIGN.md 4.6 (``survey``: of 4.8, not periodic, with the observer at the origin; 'angular' takes unit vectors and
+    chord edges).  pos: (n, 3) float32 / float64 device tensors in box coordinates; w: float64 (n,).  Returns device
     tensors (npairs int64, wsum f64, sepsum f64) of nbins entries and the number of candidate pairs tested."""
     dev = pos1.device
     axes = [i for i in range(3) if i != los] + [los]
@@ -141,8 +144,9 @@ def count_pairs(mode, pos1, w1, pos2, w2, edges, periodic, box, los=2, Nmu=None,
         del p1
         first, ckey, nchunks = c1.chunks(int(lib().nbk_paircount_chunk_rows()))
     work = torch.empty(len(e1) + (2 if e2 is None else len(e2)), dtype=torch.float64, device=dev)
+    kmode = (_SURVEY_KERNEL_MODES if survey else _MODES)[mode]
     with stage("paircount_count"):
-        check(lib().nbk_paircount(_MODES[mode], _ptr(c1.pos), _ptr(c1.w), _ptr(first), _ptr(ckey), nchunks, _ptr(c2.pos), _ptr(c2.w),
+        check(lib().nbk_paircount(kmode, _ptr(c1.pos), _ptr(c1.w), _ptr(first), _ptr(ckey), nchunks, _ptr(c2.pos), _ptr(c2.w),
                                   _ptr(c2.cell_start), _ptr(c2.cell_key), c2.ncells, int(periodic), darr(gbox), iarr(ncell),
                                   darr(tol), darr(e1), len(e1), darr(e2) if e2 is not None else None,
                                   len(e2) if e2 is not None else 0, float(pimax or 0.0), _ptr(work), _ptr(npairs), _ptr(wsum),
@@ -194,8 +198,25 @@ def slab_route(comm, pos1, w1, pos2, w2, periodic, box, smax):
     return prim.contiguous(), pw.contiguous(), sec.contiguous(), sw.contiguous()
 
 
-def _verify_sources(first, second, BoxSize, columns):
-    """the box of the count from the sources' attrs and the `BoxSize` keyword; every source must hold `columns`"""
+def reduce_histograms(comm, npairs, wsum, ssum, cand):
+    """host arrays of the count_pairs histograms summed over ranks, in one all-reduce (counts as two exact 32-bit
+    halves)"""
+    if comm.size == 1:
+        return npairs.cpu().numpy().astype('u8'), wsum.cpu().numpy(), ssum.cpu().numpy(), int(cand)
+    c = torch.cat([npairs, torch.tensor([cand], dtype=torch.int64, device=npairs.device)])
+    packed = torch.cat([(c & 0xffffffff).to(torch.float64), (c >> 32).to(torch.float64), wsum, ssum])
+    comm.allreduce_tensor(packed, "sum")
+    k = c.shape[0]
+    lo = packed[:k].round().to(torch.int64)
+    hi = packed[k:2 * k].round().to(torch.int64)
+    tot = (hi << 32) + lo
+    nb = npairs.shape[0]
+    return (tot[:nb].cpu().numpy().astype('u8'), packed[2 * k:2 * k + nb].cpu().numpy(),
+            packed[2 * k + nb:].cpu().numpy(), int(tot[nb].item()))
+
+
+def _verify_columns(first, second, columns):
+    """both sources (second None: the first) share a communicator and hold `columns`"""
     if second is None:
         second = first
     assert second.comm is first.comm, "communicator mismatch between input sources"
@@ -203,6 +224,25 @@ def _verify_sources(first, second, BoxSize, columns):
         for col in columns:
             if col not in source:
                 raise ValueError("the column '%s' is missing from input source; cannot do pair count" % col)
+
+
+def weight_column(source, name):
+    """a source's weight column as a contiguous float64 (n,) tensor on the GPU"""
+    col = source[name]
+    if hasattr(col, 'materialize'):
+        col = col.materialize()
+    col = col.compute() if hasattr(col, 'compute') else col
+    t = torch.as_tensor(col)
+    if not t.is_cuda:
+        t = t.cuda()
+    return t.to(torch.float64).reshape(-1).contiguous()
+
+
+def _verify_sources(first, second, BoxSize, columns):
+    """the box of the count from the sources' attrs and the `BoxSize` keyword; every source must hold `columns`"""
+    _verify_columns(first, second, columns)
+    if second is None:
+        second = first
     box = numpy.zeros(3)
     b1 = first.attrs.get('BoxSize', None)
     b2 = second.attrs.get('BoxSize', None)
@@ -220,7 +260,65 @@ def _verify_sources(first, second, BoxSize, columns):
     return box
 
 
-class SimulationBoxPairCount(object):
+def check_pair_args(mode, edges, Nmu, pimax):
+    """the argument checks of the reference's PairCountBase, and those of the bin edges (as float64, returned)"""
+    if mode not in ['1d', '2d', 'projected', 'angular']:
+        raise ValueError("allowed 'mode' values are: %s" % ['1d', '2d', 'projected', 'angular'])
+    if numpy.min(edges) <= 0.:
+        raise ValueError("the lower edge of the 1st separation bin must greater than zero (no self-pairs)")
+    if mode == '2d' and Nmu is None:
+        raise ValueError("'Nmu' keyword is required when 'mode' is '2d'")
+    if Nmu is not None and mode != '2d':
+        raise ValueError("mode should be '2d' if 'Nmu' is specified")
+    if mode == 'projected' and pimax is None:
+        raise ValueError("'pimax' keyword is required when 'mode' is 'projected'")
+    if pimax is not None and mode != 'projected':
+        raise ValueError("mode should be 'projected' if 'projected' is specified")
+    if mode == 'projected' and pimax < 1.0:
+        raise ValueError("'pimax' must be at least 1.0 when 'mode' is 'projected'")
+    e = numpy.asarray(edges, dtype='f8')
+    if e.ndim != 1 or len(e) < 2 or not numpy.isfinite(e).all() or not (numpy.diff(e) > 0).all():
+        raise ValueError("pair count: edges must be a 1-D array of at least two finite, strictly increasing values")
+    if mode == '2d' and (int(Nmu) != Nmu or Nmu < 1):
+        raise ValueError("pair count: Nmu must be a positive integer")
+    return e
+
+
+class BasePairCount(object):
+    """a pair-count result (``pairs``, ``attrs``), saved and loaded as JSON; subclasses rebuild ``pairs`` in
+    ``__setstate__``"""
+
+    def __getstate__(self):
+        return {'pairs': self.pairs.data, 'attrs': self.attrs}
+
+    def save(self, output):
+        """save the result as JSON (``{'pairs': ..., 'attrs': ...}``)"""
+        import json
+        from ..utils import JSONEncoder
+        if self.comm.rank == 0:
+            self.logger.info('measurement done; saving result to %s' % output)
+            with open(output, 'w') as ff:
+                json.dump(self.__getstate__(), ff, cls=JSONEncoder)
+
+    @classmethod
+    @CurrentMPIComm.enable
+    def load(cls, output, comm=None):
+        """load a result written by :func:`save`"""
+        import json
+        from ..utils import JSONDecoder
+        if comm.rank == 0:
+            with open(output, 'r') as ff:
+                state = json.load(ff, cls=JSONDecoder)
+        else:
+            state = None
+        state = comm.bcast(state)
+        self = object.__new__(cls)
+        self.__setstate__(state)
+        self.comm = comm
+        return self
+
+
+class SimulationBoxPairCount(BasePairCount):
     r"""
     Count (weighted) pairs of objects in a simulation box as a function of :math:`r`, :math:`(r, \mu)` or
     :math:`(r_p, \pi)`, on one or several GPUs.  Runs on construction.
@@ -279,25 +377,7 @@ class SimulationBoxPairCount(object):
 
         BoxSize = _verify_sources(first, second, BoxSize, [position, weight])
 
-        if mode not in ['1d', '2d', 'projected', 'angular']:
-            raise ValueError("allowed 'mode' values are: %s" % ['1d', '2d', 'projected', 'angular'])
-        if numpy.min(edges) <= 0.:
-            raise ValueError("the lower edge of the 1st separation bin must greater than zero (no self-pairs)")
-        if mode == '2d' and Nmu is None:
-            raise ValueError("'Nmu' keyword is required when 'mode' is '2d'")
-        if Nmu is not None and mode != '2d':
-            raise ValueError("mode should be '2d' if 'Nmu' is specified")
-        if mode == 'projected' and pimax is None:
-            raise ValueError("'pimax' keyword is required when 'mode' is 'projected'")
-        if pimax is not None and mode != 'projected':
-            raise ValueError("mode should be 'projected' if 'projected' is specified")
-        if mode == 'projected' and pimax < 1.0:
-            raise ValueError("'pimax' must be at least 1.0 when 'mode' is 'projected'")
-        e = numpy.asarray(edges, dtype='f8')
-        if e.ndim != 1 or len(e) < 2 or not numpy.isfinite(e).all() or not (numpy.diff(e) > 0).all():
-            raise ValueError("pair count: edges must be a 1-D array of at least two finite, strictly increasing values")
-        if mode == '2d' and (int(Nmu) != Nmu or Nmu < 1):
-            raise ValueError("pair count: Nmu must be a positive integer")
+        check_pair_args(mode, edges, Nmu, pimax)
         if mode == 'angular':
             raise NotImplementedError("mode='angular' needs the Cartesian to RA/Dec transform (CartesianToEquatorial) "
                                       "and an angular pair counter, which nbodykit_b200 does not have")
@@ -329,14 +409,7 @@ class SimulationBoxPairCount(object):
         self.run()
 
     def _weights(self, source):
-        col = source[self.attrs['weight']]
-        if hasattr(col, 'materialize'):
-            col = col.materialize()
-        col = col.compute() if hasattr(col, 'compute') else col
-        t = torch.as_tensor(col)
-        if not t.is_cuda:
-            t = t.cuda()
-        return t.to(torch.float64).reshape(-1).contiguous()
+        return weight_column(source, self.attrs['weight'])
 
     def run(self):
         """count the pairs; sets :attr:`pairs` and ``attrs['total_wnpairs']`` / ``attrs['is_cross']``"""
@@ -399,24 +472,9 @@ class SimulationBoxPairCount(object):
 
     def _reduce(self, npairs, wsum, ssum, cand):
         """host arrays of the histograms summed over ranks, in one all-reduce (counts as two exact 32-bit halves)"""
-        comm = self.comm
-        if comm.size == 1:
-            return npairs.cpu().numpy().astype('u8'), wsum.cpu().numpy(), ssum.cpu().numpy(), int(cand)
-        c = torch.cat([npairs, torch.tensor([cand], dtype=torch.int64, device=npairs.device)])
-        packed = torch.cat([(c & 0xffffffff).to(torch.float64), (c >> 32).to(torch.float64), wsum, ssum])
-        comm.allreduce_tensor(packed, "sum")
-        k = c.shape[0]
-        lo = packed[:k].round().to(torch.int64)
-        hi = packed[k:2 * k].round().to(torch.int64)
-        tot = (hi << 32) + lo
-        nb = npairs.shape[0]
-        return (tot[:nb].cpu().numpy().astype('u8'), packed[2 * k:2 * k + nb].cpu().numpy(),
-                packed[2 * k + nb:].cpu().numpy(), int(tot[nb].item()))
+        return reduce_histograms(self.comm, npairs, wsum, ssum, cand)
 
     # ------------------------------------------------------------------------------------------------------------------
-    def __getstate__(self):
-        return {'pairs': self.pairs.data, 'attrs': self.attrs}
-
     def __setstate__(self, state):
         self.__dict__.update(state)
         a = self.attrs
@@ -424,32 +482,6 @@ class SimulationBoxPairCount(object):
             raise ValueError("mode = '%s' should be one of %s" % (a['mode'], list(_MODES)))
         dims, edges = _dims_edges(a['mode'], a['edges'], a['Nmu'], a['pimax'])
         self.pairs = BinnedStatistic(dims, edges, self.pairs, fields_to_sum=['npairs', 'wnpairs'])
-
-    def save(self, output):
-        """save the result as JSON (``{'pairs': ..., 'attrs': ...}``)"""
-        import json
-        from ..utils import JSONEncoder
-        if self.comm.rank == 0:
-            self.logger.info('measurement done; saving result to %s' % output)
-            with open(output, 'w') as ff:
-                json.dump(self.__getstate__(), ff, cls=JSONEncoder)
-
-    @classmethod
-    @CurrentMPIComm.enable
-    def load(cls, output, comm=None):
-        """load a result written by :func:`save`"""
-        import json
-        from ..utils import JSONDecoder
-        if comm.rank == 0:
-            with open(output, 'r') as ff:
-                state = json.load(ff, cls=JSONDecoder)
-        else:
-            state = None
-        state = comm.bcast(state)
-        self = object.__new__(cls)
-        self.__setstate__(state)
-        self.comm = comm
-        return self
 
 
 # ---- estimators ------------------------------------------------------------------------------------------------------
@@ -557,7 +589,58 @@ def _wedge(b):
     return b if b is None or isinstance(b, WedgeBinnedStatistic) else b.copy(cls=WedgeBinnedStatistic)
 
 
-class SimulationBox2PCF(object):
+class BasePairCount2PCF(object):
+    """the result of a pair-count correlation function: ``corr``, the pair counts ``D1D2``, ``D1R2``, ``D2R1``,
+    ``R1R2`` and ``wp`` (WedgeBinnedStatistic or None), ``attrs``; saved and loaded as JSON"""
+
+    def __getstate__(self):
+        state = {'corr': self.corr.data, 'dims': self.corr.dims, 'edges': [self.corr.edges[d] for d in self.corr.dims]}
+        for name in ('D1D2', 'D1R2', 'D2R1', 'R1R2', 'wp'):
+            v = getattr(self, name, None)
+            state[name] = v.data if v is not None else None
+        state['attrs'] = self.attrs
+        return state
+
+    def __setstate__(self, state):
+        state = dict(state)
+        edges, dims = state.pop('edges'), state.pop('dims')
+        self.__dict__.update(state)
+        self.corr = WedgeBinnedStatistic(dims, edges, self.corr)
+        if self.wp is not None:
+            self.wp = WedgeBinnedStatistic(dims[:1], edges[:1], self.wp)
+        for name in ('D1D2', 'D1R2', 'D2R1', 'R1R2'):
+            v = getattr(self, name)
+            if v is not None:
+                setattr(self, name, WedgeBinnedStatistic(dims, edges, v))
+
+    def save(self, output):
+        """save the result as JSON"""
+        import json
+        from ..utils import JSONEncoder
+        if self.comm.rank == 0:
+            self.logger.info('measurement done; saving result to %s' % output)
+            with open(output, 'w') as ff:
+                json.dump(self.__getstate__(), ff, cls=JSONEncoder)
+
+    @classmethod
+    @CurrentMPIComm.enable
+    def load(cls, output, comm=None):
+        """load a result written by :func:`save`"""
+        import json
+        from ..utils import JSONDecoder
+        if comm.rank == 0:
+            with open(output, 'r') as ff:
+                state = json.load(ff, cls=JSONDecoder)
+        else:
+            state = None
+        state = comm.bcast(state)
+        self = object.__new__(cls)
+        self.__setstate__(state)
+        self.comm = comm
+        return self
+
+
+class SimulationBox2PCF(BasePairCount2PCF):
     r"""
     The two-point correlation function of catalogues in a simulation box, from pair counts, as a function of
     :math:`r`, :math:`(r, \mu)` or :math:`(r_p, \pi)`.  Runs on construction.
@@ -617,49 +700,3 @@ class SimulationBox2PCF(object):
         for name in ('D1D2', 'D1R2', 'D2R1', 'R1R2'):
             setattr(self, name, _wedge(getattr(self, name)))
         self.wp = projected_wp(self.corr) if self.attrs['mode'] == 'projected' else None
-
-    def __getstate__(self):
-        state = {'corr': self.corr.data, 'dims': self.corr.dims, 'edges': [self.corr.edges[d] for d in self.corr.dims]}
-        for name in ('D1D2', 'D1R2', 'D2R1', 'R1R2', 'wp'):
-            v = getattr(self, name, None)
-            state[name] = v.data if v is not None else None
-        state['attrs'] = self.attrs
-        return state
-
-    def __setstate__(self, state):
-        state = dict(state)
-        edges, dims = state.pop('edges'), state.pop('dims')
-        self.__dict__.update(state)
-        self.corr = WedgeBinnedStatistic(dims, edges, self.corr)
-        if self.wp is not None:
-            self.wp = WedgeBinnedStatistic(dims[:1], edges[:1], self.wp)
-        for name in ('D1D2', 'D1R2', 'D2R1', 'R1R2'):
-            v = getattr(self, name)
-            if v is not None:
-                setattr(self, name, WedgeBinnedStatistic(dims, edges, v))
-
-    def save(self, output):
-        """save the result as JSON"""
-        import json
-        from ..utils import JSONEncoder
-        if self.comm.rank == 0:
-            self.logger.info('measurement done; saving result to %s' % output)
-            with open(output, 'w') as ff:
-                json.dump(self.__getstate__(), ff, cls=JSONEncoder)
-
-    @classmethod
-    @CurrentMPIComm.enable
-    def load(cls, output, comm=None):
-        """load a result written by :func:`save`"""
-        import json
-        from ..utils import JSONDecoder
-        if comm.rank == 0:
-            with open(output, 'r') as ff:
-                state = json.load(ff, cls=JSONDecoder)
-        else:
-            state = None
-        state = comm.bcast(state)
-        self = object.__new__(cls)
-        self.__setstate__(state)
-        self.comm = comm
-        return self

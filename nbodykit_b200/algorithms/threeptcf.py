@@ -31,7 +31,8 @@ from .._lib import check, darr, i32arr, iarr, lib, stage
 from ..binned_statistic import BinnedStatistic
 from ..pmesh.pm import _ptr, _stream
 from .fof import _column
-from .paircount import _CELLS_PER_SMAX, _Cells, _check_rows, _verify_sources, slab_route
+from .paircount import (_CELLS_PER_SMAX, _Cells, _check_rows, _verify_columns, _verify_sources, slab_route,
+                        weight_column)
 
 
 def max_ell():
@@ -215,14 +216,14 @@ class SimulationBox3PCF(object):
         self.poles = self.run()
 
     def _weights(self):
-        col = self.source[self.attrs['weight']]
-        if hasattr(col, 'materialize'):
-            col = col.materialize()
-        col = col.compute() if hasattr(col, 'compute') else col
-        t = torch.as_tensor(col)
-        if not t.is_cuda:
-            t = t.cuda()
-        return t.to(torch.float64).reshape(-1).contiguous()
+        return weight_column(self.source, self.attrs['weight'])
+
+    def _rows(self):
+        """(positions, float64 weights) of the catalogue on the device"""
+        pos = _column(self.source, self.attrs['position'], None)
+        if pos.ndim != 2 or pos.shape[1] != 3:
+            raise ValueError("3PCF: Position must have shape (n, 3)")
+        return pos, self._weights()
 
     def run(self, pedantic=False):
         """compute the multipoles; sets and returns :attr:`poles`, and sets :attr:`npairs` and :attr:`candidates`.
@@ -233,12 +234,9 @@ class SimulationBox3PCF(object):
         periodic = bool(attrs['periodic'])
         poles = _check_poles(attrs['poles'])
         e = _check_edges(attrs['edges'])
-        pos = _column(self.source, attrs['position'], None)
-        if pos.ndim != 2 or pos.shape[1] != 3:
-            raise ValueError("3PCF: Position must have shape (n, 3)")
-        w = self._weights()
+        pos, w = self._rows()
         _check_rows(int(pos.shape[0]), "the catalogue")
-        box = numpy.asarray(attrs['BoxSize'], 'f8')
+        box = numpy.asarray(attrs['BoxSize'], 'f8') if periodic else None
         rmax = float(e[-1])
         with stage("threeptcf_route"):
             if comm.size > 1:
@@ -310,3 +308,61 @@ class SimulationBox3PCF(object):
         self.__setstate__(state)
         self.comm = comm
         return self
+
+
+class SurveyData3PCF(SimulationBox3PCF):
+    r"""
+    The multipoles :math:`\zeta_\ell(r_1, r_2)` of the isotropic three-point correlation function of a survey
+    catalogue, on one or several GPUs.  Runs on construction.
+
+    The RA, Dec (degrees) and redshift columns are converted to Cartesian positions with
+    :func:`~nbodykit_b200.transform.SkyToCartesian` (observer at the origin), which are then treated as
+    :class:`SimulationBox3PCF` with ``periodic=False`` treats its positions: the result equals that of the
+    non-periodic box on the same rows.
+
+    Parameters
+    ----------
+    source : CatalogSource
+        the catalogue; it provides both the primaries and the secondaries
+    poles : list of int
+        the multipoles to compute, distinct, from 0 up to :func:`max_ell`
+    edges : array_like
+        the radial bin edges in Mpc/h (see :class:`SimulationBox3PCF`)
+    cosmo : Cosmology
+        converts redshift into comoving distance (any object with ``comoving_distance(z)``)
+    domain_factor : int, optional
+        recorded in :attr:`attrs`; it has no effect (ranks take equal-width x slabs)
+    ra, dec, redshift, weight : str, optional
+        the column names
+
+    Attributes
+    ----------
+    poles, npairs, candidates :
+        as :class:`SimulationBox3PCF`
+    """
+    logger = logging.getLogger("SurveyData3PCF")
+
+    def __init__(self, source, poles, edges, cosmo, domain_factor=4, ra='RA', dec='DEC', redshift='Redshift',
+                 weight='Weight'):
+        _verify_columns(source, None, [ra, dec, redshift, weight])
+        p = _check_poles(poles)
+        _check_edges(edges)
+        self.source = source
+        self.comm = source.comm
+        self.attrs = {}
+        self.attrs['poles'] = p
+        self.attrs['edges'] = edges
+        self.attrs['cosmo'] = cosmo
+        self.attrs['periodic'] = False
+        self.attrs['weight'] = weight
+        self.attrs['ra'] = ra
+        self.attrs['dec'] = dec
+        self.attrs['redshift'] = redshift
+        self.attrs['domain_factor'] = domain_factor
+        self.poles = self.run()
+
+    def _rows(self):
+        from .surveypaircount import sky_rows
+        a = self.attrs
+        pos = sky_rows(self.source, a['ra'], a['dec'], a['redshift'], a['cosmo'], self.comm, "SurveyData3PCF")
+        return pos, self._weights().to(pos.device)

@@ -59,7 +59,7 @@ __global__ void __launch_bounds__(PC_B, 4) k_paircount(const double *__restrict_
         for (int b = threadIdx.x; b < nbins; b += PC_B) { cnt[b] = 0ull; wsum[b] = 0.0; ssum[b] = 0.0; }
     }
     for (int k = threadIdx.x; k <= g.nb; k += PC_B) e2[k] = e2_g[k];
-    if (MODE != NBK_PC_1D)
+    if (MODE != NBK_PC_1D && MODE != NBK_PC_ANGULAR)
         for (int k = threadIdx.x; k <= g.n2; k += PC_B) e2nd[k] = e2nd_g[k];
 
     const int64_t c = blockIdx.x;
@@ -125,7 +125,35 @@ __global__ void __launch_bounds__(PC_B, 4) k_paircount(const double *__restrict_
                             dc = fmin(dc, g.box[2] - dc);
                         }
                         const double rp2 = da * da + db * db;
-                        if (MODE == NBK_PC_PROJECTED) {
+                        if (MODE == NBK_PC_SURVEY_2D || MODE == NBK_PC_SURVEY_PROJECTED) {
+                            // the line of sight of the pair is its midpoint: l = x1 + x2, observer at the origin
+                            const double s2 = rp2 + dc * dc;
+                            if (MODE == NBK_PC_SURVEY_2D ? (s2 < emin2 || !(s2 < emax2)) : !(s2 < g.thr_sph)) continue;
+                            const double sx = tile[j] - px, sy = tile[PC_B + j] - py, sz = tile[2 * PC_B + j] - pz;
+                            const double lx = px + tile[j], ly = py + tile[PC_B + j], lz = pz + tile[2 * PC_B + j];
+                            const double l2 = (lx * lx + ly * ly) + lz * lz;
+                            const double sl = (sx * lx + sy * ly) + sz * lz;
+                            if (MODE == NBK_PC_SURVEY_2D) {
+                                const double s = sqrt(s2);
+                                const double mu = l2 > 0.0 ? fabs(sl) / (s * sqrt(l2)) : 0.0;
+                                const int b = pc_bin(e2, g.nb, s2) * g.n2 + pc_bin(e2nd, g.n2, mu);
+                                pc_add<SMEM>(b, pwt * tile[3 * PC_B + j], s, cnt, wsum, ssum);
+                            } else {
+                                const double pi = l2 > 0.0 ? fabs(sl) / sqrt(l2) : 0.0;
+                                if (!(pi < g.pimax)) continue;
+                                double rq2 = s2 - pi * pi;
+                                rq2 = rq2 > 0.0 ? rq2 : 0.0;
+                                if (rq2 < emin2 || !(rq2 < emax2)) continue;
+                                const int b = pc_bin(e2, g.nb, rq2) * g.n2 + pc_bin(e2nd, g.n2, pi);
+                                pc_add<SMEM>(b, pwt * tile[3 * PC_B + j], sqrt(rq2), cnt, wsum, ssum);
+                            }
+                        } else if (MODE == NBK_PC_ANGULAR) {
+                            // unit vectors: bins of the chord, summed as the angle in degrees
+                            const double s2 = rp2 + dc * dc;
+                            if (s2 < emin2 || !(s2 < emax2)) continue;
+                            const double theta = 2.0 * asin(0.5 * sqrt(s2)) * (180.0 / M_PI);
+                            pc_add<SMEM>(pc_bin(e2, g.nb, s2), pwt * tile[3 * PC_B + j], theta, cnt, wsum, ssum);
+                        } else if (MODE == NBK_PC_PROJECTED) {
                             if (!(dc < g.pimax) || rp2 < emin2 || !(rp2 < emax2)) continue;
                             const int b = pc_bin(e2, g.nb, rp2) * g.n2 + pc_bin(e2nd, g.n2, dc);
                             pc_add<SMEM>(b, pwt * tile[3 * PC_B + j], sqrt(rp2), cnt, wsum, ssum);
@@ -177,7 +205,11 @@ extern "C" int nbk_paircount(int mode, const double *ppos, const double *pw, con
                              const int64_t *ncell_host, const double *tol_host, const double *edges_host, int nedges,
                              const double *edges2_host, int nedges2, double pimax, double *work, uint64_t *npairs, double *wsum,
                              double *ssum, uint64_t *candidates, void *stream) {
-    NBK_CHECK_ARG(mode == NBK_PC_1D || mode == NBK_PC_2D || mode == NBK_PC_PROJECTED, "paircount: bad mode %d", mode);
+    NBK_CHECK_ARG(mode >= NBK_PC_1D && mode <= NBK_PC_ANGULAR, "paircount: bad mode %d", mode);
+    const bool survey = mode >= NBK_PC_SURVEY_2D;
+    const bool projected = mode == NBK_PC_PROJECTED || mode == NBK_PC_SURVEY_PROJECTED;
+    const bool one_dim = mode == NBK_PC_1D || mode == NBK_PC_ANGULAR;
+    NBK_CHECK_ARG(!(survey && periodic), "paircount: mode %d (survey / angular) is not periodic", mode);
     NBK_CHECK_ARG(nchunks >= 0 && nchunks < (1ll << 31), "paircount: chunk count %lld out of range", (long long)nchunks);
     NBK_CHECK_ARG(nscells >= 0 && nscells < (1ll << 32), "paircount: cell count %lld out of range", (long long)nscells);
     NBK_CHECK_ARG(box_host != nullptr && ncell_host != nullptr && tol_host != nullptr && edges_host != nullptr,
@@ -192,7 +224,7 @@ extern "C" int nbk_paircount(int mode, const double *ppos, const double *pw, con
     g.periodic = periodic ? 1 : 0;
     g.nb = nedges - 1;
     g.n2 = 1;
-    if (mode != NBK_PC_1D) {
+    if (!one_dim) {
         NBK_CHECK_ARG(edges2_host != nullptr && nedges2 >= 2 && nedges2 <= PC_MAX_EDGES,
                       "paircount: %d second-dimension edges (2 .. %d supported)", nedges2, PC_MAX_EDGES);
         g.n2 = nedges2 - 1;
@@ -201,12 +233,13 @@ extern "C" int nbk_paircount(int mode, const double *ppos, const double *pw, con
     const double emax = edges_host[nedges - 1];
     double smax2 = emax * emax;
     g.pimax = 0.0;
-    if (mode == NBK_PC_PROJECTED) {
+    if (projected) {
         NBK_CHECK_ARG(isfinite(pimax) && pimax > 0, "paircount: pimax must be positive and finite (got %g)", pimax);
         g.pimax = pimax;
         smax2 = smax2 + pimax * pimax;
     }
-    // the skip thresholds: a relative margin far above the rounding of the gaps and of the pair separations
+    // the skip thresholds: a relative margin far above the rounding of the gaps and of the pair separations.  A survey
+    // pair's line of sight is its own, so survey 'projected' prunes on the sphere s_max^2 = r_p,max^2 + pimax^2.
     g.thr_xy = (mode == NBK_PC_PROJECTED ? emax * emax : smax2) * (1.0 + 1e-9);
     g.thr_sph = smax2 * (1.0 + 1e-9);
     const double smax = sqrt(smax2);
@@ -234,7 +267,7 @@ extern "C" int nbk_paircount(int mode, const double *ppos, const double *pw, con
     double *hbuf = (double *)malloc(sizeof(double) * ((g.nb + 1) + (g.n2 + 1)));
     NBK_CHECK_ARG(hbuf != nullptr, "paircount: out of host memory");
     for (int k = 0; k <= g.nb; k++) hbuf[k] = edges_host[k] * edges_host[k];
-    for (int k = 0; k <= g.n2; k++) hbuf[g.nb + 1 + k] = mode == NBK_PC_1D ? 0.0 : edges2_host[k];
+    for (int k = 0; k <= g.n2; k++) hbuf[g.nb + 1 + k] = one_dim ? 0.0 : edges2_host[k];
     cudaError_t e = cudaMemcpyAsync(work, hbuf, sizeof(double) * ((g.nb + 1) + (g.n2 + 1)), cudaMemcpyHostToDevice, s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
     free(hbuf);
@@ -246,6 +279,10 @@ extern "C" int nbk_paircount(int mode, const double *ppos, const double *pw, con
 #define PC_GO(M, S) pc_launch<M, S>(nchunks, shm, s, ppos, pw, cf, ck, spos, sw, scs, sck, nscells, g, e2, e2nd, cnt, wsum, ssum, cand)
     if (mode == NBK_PC_1D) return smem ? PC_GO(NBK_PC_1D, true) : PC_GO(NBK_PC_1D, false);
     if (mode == NBK_PC_2D) return smem ? PC_GO(NBK_PC_2D, true) : PC_GO(NBK_PC_2D, false);
-    return smem ? PC_GO(NBK_PC_PROJECTED, true) : PC_GO(NBK_PC_PROJECTED, false);
+    if (mode == NBK_PC_PROJECTED) return smem ? PC_GO(NBK_PC_PROJECTED, true) : PC_GO(NBK_PC_PROJECTED, false);
+    if (mode == NBK_PC_SURVEY_2D) return smem ? PC_GO(NBK_PC_SURVEY_2D, true) : PC_GO(NBK_PC_SURVEY_2D, false);
+    if (mode == NBK_PC_SURVEY_PROJECTED)
+        return smem ? PC_GO(NBK_PC_SURVEY_PROJECTED, true) : PC_GO(NBK_PC_SURVEY_PROJECTED, false);
+    return smem ? PC_GO(NBK_PC_ANGULAR, true) : PC_GO(NBK_PC_ANGULAR, false);
 #undef PC_GO
 }

@@ -12,11 +12,11 @@ struct PcGeom {
     long long nc[3];    // cells per axis
     long long reach[3]; // largest cell-index difference of a pair within s_max
     int periodic;
-    int mode;           // NBK_PC_1D / 2D / PROJECTED
+    int mode;           // NBK_PC_1D / 2D / PROJECTED / SURVEY_2D / SURVEY_PROJECTED / ANGULAR
     int nb;             // bins along the first dimension (edges: nb + 1)
-    int n2;             // bins along the second dimension (mu or pi; 1 in '1d')
+    int n2;             // bins along the second dimension (mu or pi; 1 in '1d' and 'angular')
     double thr_xy;      // skip a column when its smallest squared transverse gap reaches this
-    double thr_sph;     // '1d' / '2d': skip a cell when its smallest squared gap reaches this
+    double thr_sph;     // all but box 'projected': skip a cell when its smallest squared gap reaches this
     double pimax;       // 'projected': pairs need |dc| < pimax
 };
 

@@ -16,9 +16,13 @@ def attrs_to_dict(obj, prefix):
 
 class JSONEncoder(json.JSONEncoder):
     """numpy arrays -> {'__dtype__', '__shape__', '__data__'}; complex -> {'__complex__': [re, im]};
-    numpy scalars -> python scalars.  Same wire format as the reference (utils.py:381-433)."""
+    numpy scalars -> python scalars; a Cosmology -> {'__cosmo__': pars}.  Same wire format as the reference
+    (utils.py:381-433)."""
 
     def default(self, obj):
+        from .cosmology import Cosmology
+        if isinstance(obj, Cosmology):
+            return {'__cosmo__': obj.pars.copy()}
         if isinstance(obj, (complex, numpy.complexfloating)):
             return {'__complex__': [float(obj.real), float(obj.imag)]}
         if isinstance(obj, numpy.ndarray):
@@ -58,6 +62,9 @@ class JSONDecoder(json.JSONDecoder):
         if '__complex__' in value:
             re, im = value['__complex__']
             return re + 1j * im
+        if '__cosmo__' in value:
+            from .cosmology import Cosmology
+            return Cosmology.from_dict(value['__cosmo__'])
         return value
 
     def __init__(self, *args, **kwargs):
