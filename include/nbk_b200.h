@@ -419,6 +419,37 @@ int nbk_threeptcf(const double *ppos, const double *pw, const int64_t *chunk_fir
                   int nedges, const int *poles_host, int npoles, const double *coef_host, double *work, double *zeta,
                   uint64_t *npairs, uint64_t *candidates, void *stream);
 
+/* Cylindrical groups (algorithms/cgm.py: CylindricalGroups; DESIGN.md 4.9).  Rows key-sorted on a grid of ncell_host[d]
+ * cells of side box[d] / ncell[d] as for nbk_paircount: spos double [n][3] (periodic: already wrapped), sprio[n] the
+ * distinct global priority of each sorted row, perm[n] its row before sorting; rows with perm < n_own are owned, the
+ * others are copies.  Chunks of at most nbk_cgm_chunk_rows() sorted rows of one cell.  Rows a != b (a the higher
+ * priority) are linked iff |dr2 - rlos2| <= rperp^2 and rlos2 <= rpar^2, dr = x_a - x_b (periodic: minimum image with
+ * dr > L/2 -> dr - L, dr <= -L/2 -> dr + L), dr2 = (dx^2 + dy^2) + dz^2; los_host (a 3-vector): rlos2 = t^2 with
+ * t = (dx lx + dy ly) + dz lz; los_host NULL: c = (x_a + x_b) / 2, rlos2 = ((dx cx + dy cy) + dz cz)^2 / |c|^2 and no
+ * link when |c|^2 = 0.  Everything in double.
+ *   count  : counts[i] = higher-priority rows linked to owned sorted row i (copies: untouched); *candidates += pairs tested
+ *   write  : their sorted row indices at nbr[offsets[i] ..] (offsets: exclusive scan of counts, n + 1 entries)
+ *   resolve: one round over order[n_own] (owned sorted rows, descending priority) of state (0 undecided, 1 central,
+ *            2 satellite, per sorted row): undecided rows with a central neighbour become satellites, those whose
+ *            neighbours are all satellites (or none) centrals; *undecided += owned rows left undecided
+ *   assign : cen_prio[r] = the priority of the central of owned row r (its own for a central), nsat[central] += 1 per
+ *            satellite (uint64, per sorted row, zero first). */
+int64_t nbk_cgm_chunk_rows(void);
+int nbk_cgm_count(const double *spos, const int64_t *sprio, const uint32_t *perm, int64_t n, int64_t n_own,
+                  const int64_t *chunk_first, const int64_t *chunk_key, int64_t nchunks, const uint32_t *cell_start,
+                  const int64_t *cell_key, int64_t ncells, int periodic, const double *box_host, const int64_t *ncell_host,
+                  const double *tol_host, const double *los_host, double rperp, double rpar, int64_t *counts,
+                  uint64_t *candidates, void *stream);
+int nbk_cgm_write(const double *spos, const int64_t *sprio, const uint32_t *perm, int64_t n, int64_t n_own,
+                  const int64_t *chunk_first, const int64_t *chunk_key, int64_t nchunks, const uint32_t *cell_start,
+                  const int64_t *cell_key, int64_t ncells, int periodic, const double *box_host, const int64_t *ncell_host,
+                  const double *tol_host, const double *los_host, double rperp, double rpar, const int64_t *offsets,
+                  int32_t *nbr, void *stream);
+int nbk_cgm_resolve(const int32_t *order, int64_t n_own, const int64_t *offsets, const int32_t *nbr, uint8_t *state,
+                    uint64_t *undecided, void *stream);
+int nbk_cgm_assign(const int32_t *order, int64_t n_own, const int64_t *offsets, const int32_t *nbr, const uint8_t *state,
+                   const int64_t *sprio, int64_t *cen_prio, uint64_t *nsat, void *stream);
+
 /* elementwise helpers behind RealField/ComplexField `[...] = v`, `*= a`, `+= other`
  * (source/mesh/catalog.py:203,354,396-398; fftpower.py:128).  n counts REAL scalars. */
 int nbk_fill(void *x, int dtype, int64_t n, double value, void *stream);

@@ -24,6 +24,7 @@ SOURCES = [
     ("fof.cu", ["--fmad=false"]),
     ("paircount.cu", ["--fmad=false"]),
     ("threeptcf.cu", ["--fmad=false"]),
+    ("cgm.cu", ["--fmad=false"]),
 ]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ARCH + [ "-O3", "-lineinfo", "-std=c++17",

@@ -99,6 +99,13 @@ SIGNATURES = {
     "nbk_threeptcf_max_bins": ([], _i),
     "nbk_threeptcf": ([_vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _i, _pd, _pi64, _pd, _pd, _i, _pi, _i, _pd, _vp,
                        _vp, _vp, _vp, _vp], _i),
+    "nbk_cgm_chunk_rows": ([], _i64),
+    "nbk_cgm_count": ([_vp, _vp, _vp, _i64, _i64, _vp, _vp, _i64, _vp, _vp, _i64, _i, _pd, _pi64, _pd, _pd, _d, _d, _vp, _vp,
+                       _vp], _i),
+    "nbk_cgm_write": ([_vp, _vp, _vp, _i64, _i64, _vp, _vp, _i64, _vp, _vp, _i64, _i, _pd, _pi64, _pd, _pd, _d, _d, _vp, _vp,
+                       _vp], _i),
+    "nbk_cgm_resolve": ([_vp, _i64, _vp, _vp, _vp, _vp, _vp], _i),
+    "nbk_cgm_assign": ([_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp], _i),
     "nbk_fill": ([_vp, _i, _i64, _d, _vp], _i),
     "nbk_scale": ([_vp, _i, _i64, _d, _vp], _i),
     "nbk_axpy": ([_vp, _vp, _i, _i64, _d, _vp], _i),

@@ -91,6 +91,7 @@ class _Cells(object):
               "nbk_fof_sorted_pos")
         self.pos = spos.to(torch.float64).contiguous()           # exact: f4 -> f8 after the wrap in f4
         self.w = w.index_select(0, perm.to(torch.int64)).contiguous()
+        self.perm = perm                                          # row before sorting of every sorted row (uint32)
         self.n = n
 
     def chunks(self, rows):

@@ -388,6 +388,43 @@ class CatalogSourceBase(object):
                            resampler=resampler)
 
 
+class _RowMover(object):
+    """moves per-row tensors so that the row of global position rank[i] lands there, every rank keeping `n` rows: a
+    gather on one rank, one all-to-all per column on several"""
+
+    def __init__(self, comm, rank, n):
+        self.comm = comm
+        dev = rank.device
+        if comm.size == 1:
+            self.order = torch.empty(n, dtype=torch.int64, device=dev)
+            self.order[rank] = torch.arange(n, dtype=torch.int64, device=dev)
+            return
+        sizes = comm.allgather(int(n))
+        self.base = int(sum(sizes[:comm.rank]))
+        bounds = torch.tensor(numpy.cumsum(sizes)[:-1].tolist(), dtype=torch.int64, device=dev)
+        # rows in ascending destination position, hence grouped by destination rank
+        self.by_pos = torch.argsort(rank)
+        dest = torch.bucketize(rank.index_select(0, self.by_pos), bounds, right=True)
+        self.sendcounts = torch.bincount(dest, minlength=comm.size).cpu().tolist()
+        self.recvcounts = comm.alltoall_ints(self.sendcounts)
+        self.at = self._send(rank) - self.base
+
+    def _send(self, t):
+        send = t.index_select(0, self.by_pos).contiguous()
+        out = torch.empty((int(sum(self.recvcounts)),) + tuple(t.shape[1:]), dtype=t.dtype, device=t.device)
+        self.comm.all_to_all_single(out, send, list(self.recvcounts), list(self.sendcounts))
+        return out
+
+    def __call__(self, t):
+        if self.comm.size == 1:
+            return t.index_select(0, self.order.to(t.device))
+        dev = self.at.device
+        recv = self._send(t.to(dev))
+        out = torch.empty_like(recv)
+        out[self.at] = recv
+        return out.to(t.device)
+
+
 class CatalogSource(CatalogSourceBase):
     """a CatalogSourceBase with a fixed size and the default columns (base/catalog.py:876-1216)"""
     logger = logging.getLogger('CatalogSource')
@@ -399,6 +436,73 @@ class CatalogSource(CatalogSourceBase):
         # collective: every rank constructs the catalogue, so the global size is known from here on and
         # rank-0-only code (logging) may read `csize` without triggering a collective
         self._csize = int(self.comm.allreduce(self._size))
+
+    def sort(self, keys, reverse=False, usecols=None):
+        """
+        Return a catalogue whose rows are sorted globally, across all ranks, by the input keys (base/catalog.py:1100).
+
+        Rows are ordered lexicographically by `keys`, the first key primary, ascending (descending with `reverse`).
+        Values compare numerically (the reference orders float keys by their bit patterns, which reverses negative
+        values), and ties keep ascending global row order (the reference leaves them to mpsort).  Every rank keeps its
+        number of rows, as the reference's in-place sort does.  The keys are sorted on the GPU; on several ranks every
+        rank all-gathers the key columns, (8 K + 8) bytes per row of the whole catalogue for K keys
+        (base/ordering.py), and the columns travel to their new ranks in one all-to-all each.
+
+        Parameters
+        ----------
+        keys : str, list, tuple
+            the names of the columns to sort by: integer or floating point, one-dimensional, without NaN
+        reverse : bool, optional
+            if ``True``, sort in descending order
+        usecols : list, optional
+            the names of the columns of the returned catalogue (default: all columns)
+        """
+        from .ordering import check_no_nan, global_rank, key_tensor
+        from ..source.catalog.array import ArrayCatalog
+        if isinstance(keys, str):
+            keys = [keys]
+        keys = list(keys)
+        if len(set(keys)) != len(keys):
+            raise ValueError("duplicated sort keys")
+        bad = set(keys) - set(self.columns)
+        if len(bad):
+            raise ValueError("invalid sort keys: %s" % str(bad))
+        if usecols is not None:
+            if isinstance(usecols, str):
+                usecols = [usecols]
+            if not isinstance(usecols, (list, tuple)):
+                raise ValueError("usecols should be a list or tuple of column names")
+            bad = set(usecols) - set(self.columns)
+            if len(bad):
+                raise ValueError("invalid column names in usecols: %s" % str(bad))
+        kt = [key_tensor(self[k], k) for k in keys]
+        dev = torch.device("cuda", torch.cuda.current_device())
+        kt = [k.to(dev) for k in kt]
+        check_no_nan(self.comm, kt, keys)
+        n = self.size
+        rank = global_rank(self.comm, kt, n, dev, reverse=reverse)
+        del kt
+        names = self.columns if usecols is None else list(dict.fromkeys(usecols))
+        move = _RowMover(self.comm, rank, n)
+        data, const = {}, {}
+        for name in names:
+            col = self[name]
+            if isinstance(col, ConstantColumn):
+                const[name] = col.value
+                continue
+            a = col.compute()
+            if _is_torch(a):
+                data[name] = move(a)
+            else:
+                data[name] = move(torch.from_numpy(numpy.ascontiguousarray(a)).to(dev)).cpu().numpy()
+        if not data:
+            # only constant columns: the catalogue needs one array to know its size
+            data = {name: numpy.full(n, value) for name, value in const.items()}
+            const = {}
+        out = ArrayCatalog(data, comm=self.comm, **self.attrs)
+        for name, value in const.items():
+            out[name] = ConstantColumn(value, n)
+        return out
 
     @column(is_default=True)
     def Selection(self):
