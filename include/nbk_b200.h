@@ -450,6 +450,29 @@ int nbk_cgm_resolve(const int32_t *order, int64_t n_own, const int64_t *offsets,
 int nbk_cgm_assign(const int32_t *order, int64_t n_own, const int64_t *offsets, const int32_t *nbr, const uint8_t *state,
                    const int64_t *sprio, int64_t *cen_prio, uint64_t *nsat, void *stream);
 
+/* Nearest-neighbour distances in the periodic unit box (algorithms/kdtree.py: KDDensity; DESIGN.md 4.10).  K =
+ * nbk_kd_k() (8).  Distance of unit positions a, b in double: dx = a_x - b_x, dx > 0.5 -> dx - 1, dx < -0.5 -> dx + 1 per
+ * axis, d2 = (dx^2 + dy^2) + dz^2.
+ *   unit      : q (double [n][3]) = pos / L in the positions' dtype (float32: f4(f8(x) / L)), then numpy's q % 1 in that
+ *               dtype; a q of 1.0 becomes 0.0
+ *   cell_table: dense[k] (ncell[0] ncell[1] ncell[2] + 1 entries) = the first sorted row of cell key k, from the compact
+ *               table of nbk_fof_compact_write (cell_start[ncells + 1], cell_key[ncells])
+ *   self      : rows key-sorted on the grid of ncell_host[d] cells of side 1 / ncell[d]: spos double [n][3] in [0, 1), perm[n]
+ *               the row before sorting; rows with perm < n_own are owned, the others are copies.  kth[perm[i]] = the K-th
+ *               smallest d2 from owned sorted row i to all n rows, itself included (+inf with fewer than K rows)
+ *   query     : knn[i][0 .. K-1] = the K smallest d2 from qpos[i] (double [nq][3] in [0, 1)) to the owned rows, ascending
+ *   density   : dist[i] = sqrt(d2[i]), density[i] = 1 / (dist[i]^3 volume)
+ * self and query add the rows they test to *candidates (device uint64). */
+int64_t nbk_kd_k(void);
+int nbk_kd_unit(const void *pos, int pos_dtype, int64_t n, double L, double *q, void *stream);
+int nbk_kd_cell_table(const uint32_t *cell_start, const int64_t *cell_key, int64_t ncells, const int64_t *ncell_host,
+                      uint32_t *dense, void *stream);
+int nbk_kd_self(const double *spos, const uint32_t *perm, int64_t n, int64_t n_own, const uint32_t *dense,
+                const int64_t *ncell_host, double *kth, uint64_t *candidates, void *stream);
+int nbk_kd_query(const double *qpos, int64_t nq, const double *spos, const uint32_t *perm, int64_t n, int64_t n_own,
+                 const uint32_t *dense, const int64_t *ncell_host, double *knn, uint64_t *candidates, void *stream);
+int nbk_kd_density(const double *d2, int64_t n, double volume, double *dist, double *density, void *stream);
+
 /* elementwise helpers behind RealField/ComplexField `[...] = v`, `*= a`, `+= other`
  * (source/mesh/catalog.py:203,354,396-398; fftpower.py:128).  n counts REAL scalars. */
 int nbk_fill(void *x, int dtype, int64_t n, double value, void *stream);

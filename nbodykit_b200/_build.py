@@ -25,6 +25,7 @@ SOURCES = [
     ("paircount.cu", ["--fmad=false"]),
     ("threeptcf.cu", ["--fmad=false"]),
     ("cgm.cu", ["--fmad=false"]),
+    ("kdtree.cu", ["--fmad=false"]),
 ]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ARCH + [ "-O3", "-lineinfo", "-std=c++17",

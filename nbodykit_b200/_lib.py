@@ -106,6 +106,12 @@ SIGNATURES = {
                        _vp], _i),
     "nbk_cgm_resolve": ([_vp, _i64, _vp, _vp, _vp, _vp, _vp], _i),
     "nbk_cgm_assign": ([_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp], _i),
+    "nbk_kd_k": ([], _i64),
+    "nbk_kd_unit": ([_vp, _i, _i64, _d, _vp, _vp], _i),
+    "nbk_kd_cell_table": ([_vp, _vp, _i64, _pi64, _vp, _vp], _i),
+    "nbk_kd_self": ([_vp, _vp, _i64, _i64, _vp, _pi64, _vp, _vp, _vp], _i),
+    "nbk_kd_query": ([_vp, _i64, _vp, _vp, _i64, _i64, _vp, _pi64, _vp, _vp, _vp], _i),
+    "nbk_kd_density": ([_vp, _i64, _d, _vp, _vp, _vp], _i),
     "nbk_fill": ([_vp, _i, _i64, _d, _vp], _i),
     "nbk_scale": ([_vp, _i, _i64, _d, _vp], _i),
     "nbk_axpy": ([_vp, _vp, _i, _i64, _d, _vp], _i),
