@@ -473,6 +473,42 @@ int nbk_kd_query(const double *qpos, int64_t nq, const double *spos, const uint3
                  const uint32_t *dense, const int64_t *ncell_host, double *knn, uint64_t *candidates, void *stream);
 int nbk_kd_density(const double *d2, int64_t n, double volume, double *dist, double *density, void *stream);
 
+/* Fiber collisions (algorithms/fibercollisions.py: FiberCollisions; DESIGN.md 4.11).  The members of the FOF groups of
+ * at least 2 rows, sorted by (label, global row): pos float [n][3] (unit-sphere positions + 1.1, cast to float32), grow
+ * int64 [n] their global rows, gstart int64 [groups + 1] the first member of every group.  Members a, b collide when
+ * sqrt((dx^2 + dy^2) + dz^2) <= rad, in double from the float32 positions.  The greedy of a group removes, among the alive
+ * members with the most alive colliders (n_coll) and then the fewest colliders of those colliders (n_other), the
+ * ((h >> 32) k) >> 32-th of the k candidates in member order, h = SplitMix64 of (seed, the group's first global row,
+ * removals so far); it stops when no alive member has a collider.  collided (int32 [n], zeroed) gets 1 and neighbor (int64
+ * [n], -1) the global row of the nearest uncollided member (the first in member order on a tie) of every removed member.
+ *   pairs       : the groups gid[0 .. ng-1] of exactly 2 members: the pick of the two, without a distance test
+ *   small       : the groups gid[0 .. ng-1] of 3 .. nbk_fc_warp_members() members, one warp each
+ *   larger groups q = 0 .. nlg-1: member m of q is l = lbeg[q] + m (lq[l] = q), at segment row lseg[q] + m
+ *   cell_keys   : keys[l] of segment row lrow[l] on nc^3 cells of side cs >= rad over [0, nc cs)^3
+ *   count/write : counts[l] = colliders of l, then their group-local indices at nbr[offsets[l] ..]; cidx / ckey are the l
+ *                 sorted by (q, key) and their keys
+ *   greedy      : one block per group; groups above nbk_fc_smem_members() members keep their state in the scratch arrays
+ *                 (indexed by l); nunc[q] = members left uncollided
+ *   nearest     : the neighbor of every collided member of the larger groups, by a walk over rings of cells
+ * small and greedy add their removals to *steps, and count the members it tests to *candidates (device uint64). */
+int64_t nbk_fc_warp_members(void);
+int64_t nbk_fc_smem_members(void);
+int nbk_fc_pairs(const int64_t *gstart, const int32_t *gid, int64_t ng, const int64_t *grow, uint64_t seed, int32_t *collided,
+                 int64_t *neighbor, void *stream);
+int nbk_fc_small(const float *pos, const int64_t *gstart, const int32_t *gid, int64_t ng, const int64_t *grow, double rad,
+                 uint64_t seed, int32_t *collided, int64_t *neighbor, uint64_t *steps, void *stream);
+int nbk_fc_cell_keys(const float *pos, const int64_t *lrow, int64_t nl, double cs, int64_t nc, int64_t *keys, void *stream);
+int nbk_fc_count(const float *pos, const int32_t *lq, const int64_t *lbeg, const int64_t *lseg, int64_t nl, const int32_t *cidx,
+                 const int64_t *ckey, double cs, int64_t nc, double rad, int64_t *counts, uint64_t *candidates, void *stream);
+int nbk_fc_write(const float *pos, const int32_t *lq, const int64_t *lbeg, const int64_t *lseg, int64_t nl, const int32_t *cidx,
+                 const int64_t *ckey, double cs, int64_t nc, double rad, const int64_t *offsets, int32_t *nbr, void *stream);
+int nbk_fc_greedy(const int64_t *lbeg, const int64_t *lseg, int64_t nlg, int64_t max_members, const int64_t *offsets,
+                  const int32_t *nbr, const int64_t *grow, uint64_t seed, int32_t *scratch_ncoll, int64_t *scratch_nother,
+                  uint8_t *scratch_alive, int32_t *collided, int64_t *nunc, uint64_t *steps, void *stream);
+int nbk_fc_nearest(const float *pos, const int32_t *lq, const int64_t *lbeg, const int64_t *lseg, int64_t nl, const int32_t *cidx,
+                   const int64_t *ckey, double cs, int64_t nc, const int32_t *collided, const int64_t *nunc, const int64_t *grow,
+                   int64_t *neighbor, void *stream);
+
 /* elementwise helpers behind RealField/ComplexField `[...] = v`, `*= a`, `+= other`
  * (source/mesh/catalog.py:203,354,396-398; fftpower.py:128).  n counts REAL scalars. */
 int nbk_fill(void *x, int dtype, int64_t n, double value, void *stream);

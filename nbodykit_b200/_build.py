@@ -26,6 +26,7 @@ SOURCES = [
     ("threeptcf.cu", ["--fmad=false"]),
     ("cgm.cu", ["--fmad=false"]),
     ("kdtree.cu", ["--fmad=false"]),
+    ("fibercollisions.cu", ["--fmad=false"]),
 ]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ARCH + [ "-O3", "-lineinfo", "-std=c++17",

@@ -112,6 +112,15 @@ SIGNATURES = {
     "nbk_kd_self": ([_vp, _vp, _i64, _i64, _vp, _pi64, _vp, _vp, _vp], _i),
     "nbk_kd_query": ([_vp, _i64, _vp, _vp, _i64, _i64, _vp, _pi64, _vp, _vp, _vp], _i),
     "nbk_kd_density": ([_vp, _i64, _d, _vp, _vp, _vp], _i),
+    "nbk_fc_warp_members": ([], _i64),
+    "nbk_fc_smem_members": ([], _i64),
+    "nbk_fc_pairs": ([_vp, _vp, _i64, _vp, ctypes.c_uint64, _vp, _vp, _vp], _i),
+    "nbk_fc_small": ([_vp, _vp, _vp, _i64, _vp, _d, ctypes.c_uint64, _vp, _vp, _vp, _vp], _i),
+    "nbk_fc_cell_keys": ([_vp, _vp, _i64, _d, _i64, _vp, _vp], _i),
+    "nbk_fc_count": ([_vp, _vp, _vp, _vp, _i64, _vp, _vp, _d, _i64, _d, _vp, _vp, _vp], _i),
+    "nbk_fc_write": ([_vp, _vp, _vp, _vp, _i64, _vp, _vp, _d, _i64, _d, _vp, _vp, _vp], _i),
+    "nbk_fc_greedy": ([_vp, _vp, _i64, _i64, _vp, _vp, _vp, ctypes.c_uint64, _vp, _vp, _vp, _vp, _vp, _vp, _vp], _i),
+    "nbk_fc_nearest": ([_vp, _vp, _vp, _vp, _i64, _vp, _vp, _d, _i64, _vp, _vp, _vp, _vp, _vp], _i),
     "nbk_fill": ([_vp, _i, _i64, _d, _vp], _i),
     "nbk_scale": ([_vp, _i, _i64, _d, _vp], _i),
     "nbk_axpy": ([_vp, _vp, _i, _i64, _d, _vp], _i),
