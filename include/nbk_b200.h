@@ -509,6 +509,27 @@ int nbk_fc_nearest(const float *pos, const int32_t *lq, const int64_t *lbeg, con
                    const int64_t *ckey, double cs, int64_t nc, const int32_t *collided, const int64_t *nunc, const int64_t *grow,
                    int64_t *neighbor, void *stream);
 
+/* Redshift histogram n(z) (algorithms/zhist.py: RedshiftHistogram; DESIGN.md 4.12).  z (and w) are float32 or float64
+ * (NBK_F4 / NBK_F8), widened exactly to double; n rows, 64-bit.
+ *   moments : out[6] (device double) = count, mean, M2 (sum of squared deviations from the mean), min and max of the
+ *             finite rows, and the number of non-finite rows.  partial: device scratch of nbk_zh_partials() * 6 doubles.
+ *             The merge order depends on n alone: the same rows give the same bits on every run
+ *   bin     : counts[i] (uint64 [nb], zeroed) += the rows with edges[i] <= z < edges[i+1] (edges double [nb + 1],
+ *             non-decreasing; NaN and rows outside [edges[0], edges[nb]) are not counted); sums[i] (double [nb],
+ *             zeroed) += their weights when w is not NULL.  inv_h > 0: the edges are evenly spaced about 1 / inv_h apart,
+ *             and the bin is guessed from (z - edges[0]) inv_h and corrected against them; inv_h = 0: binary search.
+ *             nb <= nbk_zh_smem_bins() accumulates in per-CTA shared memory, more bins in global atomics
+ *   spline  : out[i] (double) = the cubic B-spline of knots t[nt] and coefficients c (nt - 4 used) at z[i], as FITPACK's
+ *             splev with ext 0 (extrapolate), 1 (zeros), 2 (raise: the extrapolated value is written) or 3 (const);
+ *             *outside (device uint64) += the rows outside [t[3], t[nt - 4]] */
+int64_t nbk_zh_smem_bins(void);
+int64_t nbk_zh_partials(void);
+int nbk_zh_moments(const void *z, int dtype, int64_t n, double *partial, double *out, void *stream);
+int nbk_zh_bin(const void *z, int dtype, const void *w, int wdtype, int64_t n, const double *edges, int64_t nb,
+               double inv_h, uint64_t *counts, double *sums, void *stream);
+int nbk_zh_spline(const void *z, int dtype, int64_t n, const double *t, int64_t nt, const double *c, int ext, double *out,
+                  uint64_t *outside, void *stream);
+
 /* elementwise helpers behind RealField/ComplexField `[...] = v`, `*= a`, `+= other`
  * (source/mesh/catalog.py:203,354,396-398; fftpower.py:128).  n counts REAL scalars. */
 int nbk_fill(void *x, int dtype, int64_t n, double value, void *stream);

@@ -27,6 +27,7 @@ SOURCES = [
     ("cgm.cu", ["--fmad=false"]),
     ("kdtree.cu", ["--fmad=false"]),
     ("fibercollisions.cu", ["--fmad=false"]),
+    ("zhist.cu", ["--fmad=false"]),
 ]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ARCH + [ "-O3", "-lineinfo", "-std=c++17",

@@ -121,6 +121,11 @@ SIGNATURES = {
     "nbk_fc_write": ([_vp, _vp, _vp, _vp, _i64, _vp, _vp, _d, _i64, _d, _vp, _vp, _vp], _i),
     "nbk_fc_greedy": ([_vp, _vp, _i64, _i64, _vp, _vp, _vp, ctypes.c_uint64, _vp, _vp, _vp, _vp, _vp, _vp, _vp], _i),
     "nbk_fc_nearest": ([_vp, _vp, _vp, _vp, _i64, _vp, _vp, _d, _i64, _vp, _vp, _vp, _vp, _vp], _i),
+    "nbk_zh_smem_bins": ([], _i64),
+    "nbk_zh_partials": ([], _i64),
+    "nbk_zh_moments": ([_vp, _i, _i64, _vp, _vp, _vp], _i),
+    "nbk_zh_bin": ([_vp, _i, _vp, _i, _i64, _vp, _i64, _d, _vp, _vp, _vp], _i),
+    "nbk_zh_spline": ([_vp, _i, _i64, _vp, _i64, _vp, _i, _vp, _vp, _vp], _i),
     "nbk_fill": ([_vp, _i, _i64, _d, _vp], _i),
     "nbk_scale": ([_vp, _i, _i64, _d, _vp], _i),
     "nbk_axpy": ([_vp, _vp, _i, _i64, _d, _vp], _i),

@@ -5,6 +5,7 @@ from .fof import FOF
 from .cgm import CylindricalGroups
 from .kdtree import KDDensity
 from .fibercollisions import FiberCollisions
+from .zhist import RedshiftHistogram
 from .paircount import SimulationBoxPairCount, SimulationBox2PCF
 from .threeptcf import SimulationBox3PCF, SurveyData3PCF
 from .surveypaircount import SurveyDataPairCount, SurveyData2PCF
@@ -12,6 +13,6 @@ from .convpower import ConvolvedFFTPower, FKPCatalog, FKPWeightFromNbar, FKPCata
 
 FKPPower = ConvolvedFFTPower
 
-__all__ = ['FOF', 'CylindricalGroups', 'KDDensity', 'FiberCollisions', 'SimulationBoxPairCount', 'SimulationBox2PCF', 'SimulationBox3PCF', 'SurveyDataPairCount',
+__all__ = ['FOF', 'CylindricalGroups', 'KDDensity', 'FiberCollisions', 'RedshiftHistogram', 'SimulationBoxPairCount', 'SimulationBox2PCF', 'SimulationBox3PCF', 'SurveyDataPairCount',
            'SurveyData2PCF', 'SurveyData3PCF', 'FFTCorr', 'FFTRecon', 'FFTPower', 'ProjectedFFTPower', 'FFTBase', 'project_to_basis', 'ConvolvedFFTPower', 'FKPPower', 'FKPCatalog',
            'FKPWeightFromNbar', 'FKPCatalogMesh']
