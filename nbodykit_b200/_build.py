@@ -28,6 +28,7 @@ SOURCES = [
     ("kdtree.cu", ["--fmad=false"]),
     ("fibercollisions.cu", ["--fmad=false"]),
     ("zhist.cu", ["--fmad=false"]),
+    ("hod.cu", ["--fmad=false"]),
 ]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ARCH + [ "-O3", "-lineinfo", "-std=c++17",

@@ -469,7 +469,33 @@ class FOF(object):
         return out
 
     def to_halos(self, particle_mass, cosmo, redshift, mdef='vir', posdef='cm', peakcolumn='Density'):
-        """the reference's HaloCatalog needs halotools and the cosmology stack (halo radius, concentration), which this
-        package does not carry; use :func:`find_features` for the group catalogue"""
-        raise NotImplementedError("FOF.to_halos needs nbodykit's HaloCatalog, which depends on halotools and the "
-                                  "cosmology package; they are not part of nbodykit_b200 -- use find_features()")
+        """
+        A :class:`~nbodykit_b200.source.catalog.halos.HaloCatalog` of the groups (fof.py:130-195): the centre-of-mass
+        (``posdef='cm'``) or peak (``posdef='peak'``, the rows at the maximum of ``peakcolumn``) position and velocity of
+        every group with members, and ``Mass = particle_mass * Length``, with the analytic default radius and
+        concentration at ``cosmo`` and ``redshift`` for the mass definition ``mdef``.
+
+        ``cosmo`` must be this package's :class:`~nbodykit_b200.cosmology.Cosmology`: the reference hands other
+        cosmologies (astropy's) to halotools, which is not a dependency.
+        """
+        from ..cosmology import Cosmology
+        from ..source.catalog.array import ArrayCatalog
+        from ..source.catalog.halos import HaloCatalog
+        if not isinstance(cosmo, Cosmology):
+            raise NotImplementedError("FOF.to_halos: a cosmology other than nbodykit_b200's Cosmology (got %r) is handed "
+                                      "to halotools by the reference; halotools is not a dependency of nbodykit_b200"
+                                      % (cosmo,))
+        if posdef not in ('cm', 'peak'):
+            raise ValueError("``posdef`` should be 'cm' or 'peak' (got %r)" % (posdef,))
+        features = self.find_features(peakcolumn=peakcolumn if posdef == 'peak' else None)
+        keep = numpy.asarray(features['Length'].compute()) > 0
+        prefix = 'CM' if posdef == 'cm' else 'Peak'
+        data = {k: numpy.asarray(features[k].compute())[keep] for k in features.columns
+                if k in ('CMPosition', 'CMVelocity', 'InitialPosition', 'PeakPosition', 'PeakVelocity', 'Length')}
+        data['Position'] = data[prefix + 'Position']
+        data['Velocity'] = data[prefix + 'Velocity']
+        data['Mass'] = particle_mass * data['Length']
+        attrs = dict(features.attrs)
+        attrs['particle_mass'] = particle_mass
+        halos = ArrayCatalog(data, comm=self.comm, **attrs)
+        return HaloCatalog(halos, cosmo, redshift, mdef=mdef, mass='Mass', position='Position', velocity='Velocity')

@@ -65,6 +65,12 @@ C_KMS = 299792.458                      # speed of light [km/s]
 # Omega_gamma h^2 per K^4: a_rad T^4 8 pi G / (3 c^2 (100 km/s/Mpc)^2), a_rad = 4 sigma_SB / c (CODATA 2018, SI)
 _SIGMA_SB, _C_SI, _G_SI, _MPC_M = 5.670374419e-8, 299792458.0, 6.67430e-11, 3.0856775814913673e22
 _OMEGA_G_H2_PER_K4 = (4 * _SIGMA_SB / _C_SI) * 8 * math.pi * _G_SI / (3 * _C_SI ** 2 * (1e5 / _MPC_M) ** 2)
+# the solar mass: the IAU 2015 nominal GM_sun (resolution B3) over G, in kg
+_GM_SUN_SI = 1.3271244e20
+M_SUN_KG = _GM_SUN_SI / _G_SI
+# G in (km/s)^2 Mpc / M_sun, and the critical density today in 10^10 (M_sun/h) / (Mpc/h)^3 (CLASS's unit for rho_crit)
+G_KMS2_MPC_PER_MSUN = _GM_SUN_SI / _MPC_M / 1e6
+RHO_CRIT0 = 3 * 100. ** 2 / (8 * math.pi * G_KMS2_MPC_PER_MSUN) / 1e10
 _DU = 1. / 64                           # table nodes: uniform in ln(1 + z)
 _GL_X, _GL_W = numpy.polynomial.legendre.leggauss(8)
 
@@ -124,6 +130,17 @@ class Cosmology(object):
         sqrt = _backend(z)[1]
         a1 = 1. + z
         return sqrt(((self.Omega0_r * a1 + self.Omega0_m) * a1 + self.Omega0_k) * a1 * a1 + self.Omega0_lambda)
+
+    def Omega_m(self, z):
+        r"""the matter density parameter at redshift z, :math:`\Omega_m (1+z)^3 / E(z)^2`; NumPy arrays / scalars, or
+        torch tensors (computed where they are)"""
+        a1 = 1. + z
+        return self.Omega0_m * a1 * a1 * a1 / self.efunc(z) ** 2
+
+    def rho_crit(self, z):
+        r"""the critical density :math:`3 H(z)^2 / (8 \pi G)` in :math:`10^{10} (M_\odot/h) / (\mathrm{Mpc}/h)^3`
+        (CLASS's name and unit); NumPy arrays / scalars, or torch tensors (computed where they are)"""
+        return RHO_CRIT0 * self.efunc(z) ** 2
 
     def _integral(self, z0, z1):
         """(c / 100) int_{z0}^{z1} dz / E(z) in Mpc/h, 8-point Gauss-Legendre, elementwise"""

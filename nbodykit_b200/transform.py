@@ -1,6 +1,7 @@
 """
 Sky <-> Cartesian coordinate transforms (API of nbodykit/transform.py: SkyToUnitSphere, SkyToCartesian,
-CartesianToEquatorial, CartesianToSky), in float64.
+CartesianToEquatorial, CartesianToSky) and the halo relations (HaloRadius, HaloConcentration, HaloVelocityDispersion,
+VectorProjection), in float64.
 
 The reference works on dask arrays; here the inputs may be catalogue Columns, torch tensors (computed on their
 device) or NumPy arrays, and the result is of the same kind: a Column if any input is one, else a tensor if any input
@@ -10,13 +11,17 @@ A `cosmo` may be any object with `comoving_distance(z)` (and, optionally, `efunc
 evaluated on the tensors where they are; any other cosmology is called on host float64 NumPy arrays, as the reference
 calls it, and its result is moved back to the tensors' device.
 """
+import math
+import re
+
 import numpy
 import torch
 
 from .base.catalog import Column, ConstantColumn
 from .cosmology import C_KMS, Cosmology
 
-__all__ = ['SkyToUnitSphere', 'SkyToCartesian', 'CartesianToEquatorial', 'CartesianToSky']
+__all__ = ['SkyToUnitSphere', 'SkyToCartesian', 'CartesianToEquatorial', 'CartesianToSky', 'HaloRadius', 'HaloConcentration',
+           'HaloVelocityDispersion', 'VectorProjection']
 
 
 def _check_frame(frame):
@@ -138,3 +143,65 @@ def CartesianToSky(pos, cosmo, velocity=None, observer=[0, 0, 0], zmax=100., fra
         vpec = (p * vals[1]).sum(dim=-1) / r
         z = z + vpec / C_KMS * (1 + z)
     return wrap(torch.stack((ra, dec, z), dim=0))
+
+
+# ---- halos ------------------------------------------------------------------------------------------------------------
+def _halo_inputs(name, mass, cosmo, redshift):
+    if not isinstance(cosmo, Cosmology):
+        raise NotImplementedError("%s: only nbodykit_b200's Cosmology is supported (the reference hands other "
+                                  "cosmologies to halotools and astropy, which are not dependencies)" % name)
+    return _inputs(mass, redshift)
+
+
+def _threshold(cosmo, z, mdef):
+    """the density threshold of mdef at redshift z (tensor), in M_sun/h per (proper Mpc/h)^3"""
+    rho = cosmo.rho_crit(z) * 1e10
+    if mdef == 'vir':
+        x = cosmo.Omega_m(z) - 1.
+        return (18 * math.pi ** 2 + 82 * x - 39 * x * x) * rho
+    m = re.fullmatch(r'(\d+)([cm])', mdef) if isinstance(mdef, str) else None
+    if m is None or int(m.group(1)) <= 0:
+        raise ValueError("mdef %r: expected 'vir', 'XXXc' or 'XXXm' with XXX a positive integer" % (mdef,))
+    delta = float(m.group(1))
+    return delta * rho if m.group(2) == 'c' else delta * cosmo.Omega_m(z) * rho
+
+
+def HaloRadius(mass, cosmo, redshift, mdef='vir'):
+    r"""the proper halo radius in Mpc/h of halos of ``mass`` (M_sun/h) for the mass definition ``mdef``:
+    :math:`R = (3 M / (4 \pi \rho_\mathrm{thr}))^{1/3}` with :math:`\rho_\mathrm{thr} = \Delta \rho_c(z)` for
+    ``'XXXc'``, :math:`\Delta \Omega_m(z) \rho_c(z)` for ``'XXXm'`` and :math:`\Delta_\mathrm{vir} \rho_c(z)` for
+    ``'vir'``, with Bryan & Norman's (1998) :math:`\Delta_\mathrm{vir} = 18\pi^2 + 82x - 39x^2`,
+    :math:`x = \Omega_m(z) - 1`.  Any other ``mdef`` raises ValueError"""
+    (mass, redshift), wrap = _halo_inputs('HaloRadius', mass, cosmo, redshift)
+    rho = _threshold(cosmo, redshift, mdef)
+    return wrap((3 * mass / (4 * math.pi * rho)) ** (1. / 3))
+
+
+def HaloConcentration(mass, cosmo, redshift, mdef='vir'):
+    r"""the NFW concentration of halos of ``mass`` (M_sun/h): the virial fit of Dutton & Maccio (2014, eqs. 12-13),
+    :math:`\log_{10} c = a + b \log_{10}(M / 10^{12} M_\odot/h)` with
+    :math:`a = 0.537 + 0.488 e^{-0.718 z^{1.08}}` and :math:`b = -0.097 + 0.024 z`, for every ``mdef`` (which is
+    still validated)"""
+    (mass, redshift), wrap = _halo_inputs('HaloConcentration', mass, cosmo, redshift)
+    _threshold(cosmo, redshift, mdef)
+    a = 0.537 + (1.025 - 0.537) * torch.exp(-0.718 * redshift ** 1.08)
+    b = -0.097 + 0.024 * redshift
+    return wrap(10. ** (a + b * torch.log10(mass / 1e12)))
+
+
+def HaloVelocityDispersion(mass, cosmo, redshift, mdef='vir'):
+    r"""the velocity dispersion in km/s of halos of ``mass`` (M_sun/h), the reference's model (Evrard et al. 2008):
+    :math:`1100 (E(z) M / 10^{15})^{0.33333}`"""
+    (mass, redshift), wrap = _halo_inputs('HaloVelocityDispersion', mass, cosmo, redshift)
+    return wrap(1100. * (cosmo.efunc(redshift) * mass / 1e15) ** 0.33333)
+
+
+def VectorProjection(vector, direction):
+    r"""the components of the (..., D) ``vector`` along ``direction`` (D,):
+    :math:`(\mathbf{v} \cdot \hat{\mathbf{d}}) \hat{\mathbf{d}}` with :math:`\hat{\mathbf{d}} = \mathbf{d} / |\mathbf{d}|`
+    (``direction`` need not be normalised)"""
+    (vector,), wrap = _inputs(vector)
+    d = torch.as_tensor(numpy.asarray(direction, dtype='f8'), device=vector.device)
+    d = d / (d ** 2).sum() ** 0.5
+    proj = (vector * d).sum(dim=-1)
+    return wrap(proj[..., None] * d)
