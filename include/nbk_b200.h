@@ -530,11 +530,16 @@ int nbk_zh_bin(const void *z, int dtype, const void *w, int wdtype, int64_t n, c
 int nbk_zh_spline(const void *z, int dtype, int64_t n, const double *t, int64_t nt, const double *c, int ext, double *out,
                   uint64_t *outside, void *stream);
 
-/* Zheng07 HOD population (source/catalog/halos.py: HaloCatalog.populate; DESIGN.md 4.13).  n halos at global rows
+/* HOD population (source/catalog/halos.py: HaloCatalog.populate; DESIGN.md 4.13).  n halos at global rows
  * h0 .. h0 + n - 1; every uniform is a SplitMix64 hash of (seed, stream, global halo row, draw index).
- *   occupy : counts[i] (int64 [2 n]) = N_cen of halo i (Bernoulli, stream 0 draw 0) and counts[n + i] = N_sat (exact
- *            Poisson, stream 0 draws 1 ..), with M0 = 10^logM0, M1 = 10^logM1 and the satellite mean times the central
- *            probability when modulate is non-zero; mass (float32 / float64) in Msun/h
+ *   occupy : Zheng07.  counts[i] (int64 [2 n]) = N_cen of halo i (Bernoulli, stream 0 draw 0) and counts[n + i] = N_sat
+ *            (exact Poisson, stream 0 draws 1 ..), with M0 = 10^logM0, M1 = 10^logM1 and the satellite mean times the
+ *            central probability when modulate is non-zero; mass (float32 / float64) in Msun/h
+ *   occupy_smhm : Leauthaud11, the same draws and counts.  The cubic spline (t [nt], c, device doubles, FITPACK splev,
+ *            extrapolated) maps log10 M to the mean log10 M*; <N_cen> = erfc((threshold - log10 M*) / (sqrt 2 scatter)) / 2,
+ *            <N_sat> = (M / Msat)^alphasat exp(-Mcut / M), times <N_cen> when modulate is non-zero.  Hearin15 when pct
+ *            (double [n], the halo's percentile in its mass bin) is not NULL: both means get the Heaviside
+ *            assembly-bias shift of strength Acen / Asat (in [-1, 1]) up for pct > split, down otherwise
  *   scan   : offsets (int64 [n2 + 1]) = 0 and the inclusive sum of the n2 counts; work: nbk_hod_scan_workspace(n2) bytes
  *   emit   : galaxy row r < ngal = offsets[2 n] belongs to entry e with offsets[e] <= r < offsets[e + 1]: the central of
  *            halo e (e < n) or satellite k = r - offsets[e] of halo e - n (stream 1, draws 8 k .. 8 k + 6).  hpos, hvel,
@@ -544,6 +549,10 @@ int nbk_zh_spline(const void *z, int dtype, int64_t n, const double *t, int64_t 
 int64_t nbk_hod_scan_workspace(int64_t n2);
 int nbk_hod_occupy(const void *mass, int mdtype, int64_t n, int64_t h0, double logMmin, double sigma_logM, double M0,
                    double M1, double alpha, int modulate, uint64_t seed, int64_t *counts, void *stream);
+int nbk_hod_occupy_smhm(const void *mass, int mdtype, int64_t n, int64_t h0, const double *t, int64_t nt, const double *c,
+                        double threshold, double scatter, double Msat, double Mcut, double alphasat, int modulate,
+                        const double *pct, double split, double Acen, double Asat, uint64_t seed, int64_t *counts,
+                        void *stream);
 int nbk_hod_scan(const int64_t *counts, int64_t n2, int64_t *offsets, void *work, int64_t work_bytes, void *stream);
 int nbk_hod_emit(const int64_t *offsets, int64_t n, int64_t ngal, int64_t h0, const void *hpos, const void *hvel, int dtype,
                  const double *mass, const double *radius, const double *conc, const double *box_host, double gnewton,

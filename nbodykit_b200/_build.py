@@ -45,6 +45,7 @@ def _nvcc():
 def _stamp(path, flags):
     h = hashlib.sha1()
     for dep in [path, os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "pc_cells.cuh"),
+                os.path.join(CSRC, "splev.cuh"),
                 os.path.join(CSRC, "ylm_table.inc"),
                 os.path.join(HERE, "..", "include", "nbk_b200.h")]:
         with open(dep, "rb") as f:

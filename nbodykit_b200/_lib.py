@@ -128,6 +128,8 @@ SIGNATURES = {
     "nbk_zh_spline": ([_vp, _i, _i64, _vp, _i64, _vp, _i, _vp, _vp, _vp], _i),
     "nbk_hod_scan_workspace": ([_i64], _i64),
     "nbk_hod_occupy": ([_vp, _i, _i64, _i64, _d, _d, _d, _d, _d, _i, ctypes.c_uint64, _vp, _vp], _i),
+    "nbk_hod_occupy_smhm": ([_vp, _i, _i64, _i64, _vp, _i64, _vp, _d, _d, _d, _d, _d, _i, _vp, _d, _d, _d, ctypes.c_uint64,
+                             _vp, _vp], _i),
     "nbk_hod_scan": ([_vp, _i64, _vp, _vp, _i64, _vp], _i),
     "nbk_hod_emit": ([_vp, _i64, _i64, _i64, _vp, _vp, _i, _vp, _vp, _vp, _pd, _d, _d, _vp, _i64, _d, _d, ctypes.c_uint64,
                       _vp, _vp, _vp, _vp, _vp, _vp, _vp], _i),

@@ -1,6 +1,9 @@
-// Zheng07 HOD population of halo catalogues (source/catalog/halos.py: HaloCatalog.populate; DESIGN.md 4.13).
-//   nbk_hod_occupy : one thread per halo: the central probability and satellite mean, a Bernoulli and an exact Poisson
-//                    draw (sequential inversion below a mean of 10, Hormann's PTRS above)
+// HOD population of halo catalogues (source/catalog/halos.py: HaloCatalog.populate; DESIGN.md 4.13).
+//   nbk_hod_occupy : one thread per halo: the Zheng07 central probability and satellite mean, a Bernoulli and an exact
+//                    Poisson draw (sequential inversion below a mean of 10, Hormann's PTRS above)
+//   nbk_hod_occupy_smhm : the same draws for the Leauthaud11 means (the inverted Behroozi10 stellar-to-halo-mass relation,
+//                    a cubic spline evaluated as FITPACK's splev), with the Heaviside assembly-bias perturbation of
+//                    Hearin15 when given each halo's percentile in its mass bin
 //   nbk_hod_scan   : offsets of the galaxy rows, an inclusive sum (cub) over the 2 n counts [centrals | satellites]
 //   nbk_hod_emit   : one thread per galaxy: its halo by binary search over the offsets, then the NFW radius (the inverse of
 //                    the truncated enclosed-mass CDF, W0 Lambert), an isotropic direction, the Jeans dispersion and
@@ -9,6 +12,7 @@
 // number of ranks or the split of the rows.  The file is compiled with --fmad=false, so that every double operation
 // rounds as the float64 NumPy restatement in oracle/hod_oracle.py does.
 #include "common.cuh"
+#include "splev.cuh"
 
 #include <cub/device/device_scan.cuh>
 #include <math.h>
@@ -84,6 +88,48 @@ __global__ void __launch_bounds__(HOD_OB) k_hod_occupy(const M *__restrict__ mas
         const double p = 0.5 * (1.0 + erf((log10(m) - logMmin) / sigma_logM));
         double lam = m > M0 ? pow((m - M0) / M1, alpha) : 0.0;
         if (modulate) lam = lam * p;
+        const unsigned long long key = hod_key(seed, 0, h0 + i);
+        counts[i] = hod_uniform(key, 0) < p ? 1 : 0;
+        counts[n + i] = hod_poisson(key, lam);
+    }
+}
+
+// the Leauthaud11 / Hearin15 model: the SMHM spline (t, c) maps log10 M to the mean log10 M*, and M_sat, M_cut derive from
+// the halo mass at the threshold on the host
+struct HodSmhm {
+    double threshold, scatter, Msat, Mcut, alphasat;
+    double split, Acen, Asat;   // assembly bias: the percentile split and the strengths, in [-1, 1]
+    int modulate;
+};
+
+// the Heaviside assembly-bias mean of a halo in the upper (percentile > p) or lower part of its mass bin, for the
+// baseline mean nb with bounds [0, hi]: shifted by d up or by d (1 - p) / p down, so that the bin average stays nb when a
+// fraction 1 - p is upper; |d| is at most what keeps both means in bounds
+static __device__ __forceinline__ double hod_assembias(double nb, double A, double p, double hi, bool upper) {
+    const double r = p / (1.0 - p);
+    const double d = A >= 0.0 ? A * fmin(hi - nb, r * nb) : A * fmin(nb, r * (hi - nb));
+    const double v = upper ? nb + d : nb - (d * (1.0 - p)) / p;
+    return fmin(fmax(v, 0.0), hi);
+}
+
+template <typename M>
+__global__ void __launch_bounds__(HOD_OB) k_hod_occupy_smhm(const M *__restrict__ mass, long long n, long long h0,
+                                                            const double *__restrict__ t, int nt,
+                                                            const double *__restrict__ c, HodSmhm q,
+                                                            const double *__restrict__ pct, unsigned long long seed,
+                                                            long long *__restrict__ counts) {
+    const long long S = (long long)gridDim.x * HOD_OB;
+    for (long long i = (long long)blockIdx.x * HOD_OB + threadIdx.x; i < n; i += S) {
+        const double m = (double)mass[i];
+        const double logms = nbk_splev3(log10(m), t, nt, c);
+        double p = 0.5 * (1.0 - erf((q.threshold - logms) / (1.4142135623730951 * q.scatter)));
+        double lam = pow(m / q.Msat, q.alphasat) * exp(-q.Mcut / m);
+        if (q.modulate) lam = lam * p;
+        if (pct) {
+            const bool upper = pct[i] > q.split;
+            p = hod_assembias(p, q.Acen, q.split, 1.0, upper);
+            lam = hod_assembias(lam, q.Asat, q.split, INFINITY, upper);
+        }
         const unsigned long long key = hod_key(seed, 0, h0 + i);
         counts[i] = hod_uniform(key, 0) < p ? 1 : 0;
         counts[n + i] = hod_poisson(key, lam);
@@ -245,6 +291,34 @@ extern "C" int nbk_hod_occupy(const void *mass, int mdtype, int64_t n, int64_t h
     else
         k_hod_occupy<double><<<grid, HOD_OB, 0, s>>>((const double *)mass, n, h0, logMmin, sigma_logM, M0, M1, alpha,
                                                       modulate, seed, c);
+    NBK_LAUNCHED();
+    return NBK_OK;
+}
+
+extern "C" int nbk_hod_occupy_smhm(const void *mass, int mdtype, int64_t n, int64_t h0, const double *t, int64_t nt,
+                                   const double *c, double threshold, double scatter, double Msat, double Mcut,
+                                   double alphasat, int modulate, const double *pct, double split, double Acen, double Asat,
+                                   uint64_t seed, int64_t *counts, void *stream) {
+    NBK_CHECK_ARG(mdtype == NBK_F4 || mdtype == NBK_F8, "hod_occupy_smhm: masses must be float32 or float64");
+    NBK_CHECK_ARG(n >= 0 && h0 >= 0, "hod_occupy_smhm: %lld halos from row %lld out of range", (long long)n, (long long)h0);
+    NBK_CHECK_ARG(nt >= 2 * (NBK_SPLEV_K + 1) && nt < (1ll << 31), "hod_occupy_smhm: %lld knots out of range (at least 8)",
+                  (long long)nt);
+    NBK_CHECK_ARG(isfinite(threshold) && isfinite(scatter) && scatter > 0 && isfinite(Msat) && Msat > 0 && isfinite(Mcut) &&
+                  Mcut >= 0 && isfinite(alphasat), "hod_occupy_smhm: invalid model parameters");
+    NBK_CHECK_ARG(!pct || (split > 0 && split < 1 && fabs(Acen) <= 1 && fabs(Asat) <= 1),
+                  "hod_occupy_smhm: the split must be in (0, 1) and the assembly-bias strengths in [-1, 1]");
+    if (n == 0) return NBK_OK;
+    NBK_CHECK_ARG(mass && t && c && counts, "hod_occupy_smhm: null device array");
+    HodSmhm q;
+    q.threshold = threshold; q.scatter = scatter; q.Msat = Msat; q.Mcut = Mcut; q.alphasat = alphasat;
+    q.split = split; q.Acen = Acen; q.Asat = Asat; q.modulate = modulate;
+    cudaStream_t s = (cudaStream_t)stream;
+    const int grid = nbk_grid_for(n, HOD_OB, 8);
+    long long *cn = (long long *)counts;
+    if (mdtype == NBK_F4)
+        k_hod_occupy_smhm<float><<<grid, HOD_OB, 0, s>>>((const float *)mass, n, h0, t, (int)nt, c, q, pct, seed, cn);
+    else
+        k_hod_occupy_smhm<double><<<grid, HOD_OB, 0, s>>>((const double *)mass, n, h0, t, (int)nt, c, q, pct, seed, cn);
     NBK_LAUNCHED();
     return NBK_OK;
 }

@@ -3,11 +3,12 @@
 //                    per-thread Welford states fed with 4-row batches and merged by Chan's rule in a fixed order
 //   nbk_zh_bin     : per row the bin i with edges[i] <= z < edges[i+1] (searchsorted(edges, z, 'right') - 1), into per-CTA
 //                    shared-memory histograms flushed with global atomics, or straight into global atomics for many bins
-//   nbk_zh_spline  : a cubic B-spline (t, c) at every row, as FITPACK's splev: the knot interval, the de Boor-Cox
-//                    recurrence of fpbspl and the four extrapolation modes
+//   nbk_zh_spline  : a cubic B-spline (t, c) at every row, as FITPACK's splev (splev.cuh: the knot interval and the
+//                    de Boor-Cox recurrence of fpbspl) with its four extrapolation modes
 // Redshifts and weights are float32 or float64, widened exactly to double.  Rows are 64-bit indexed.  The file is compiled
 // with --fmad=false, so that the spline rounds as FITPACK's compiled without contraction does.
 #include "common.cuh"
+#include "splev.cuh"
 
 #include <math.h>
 
@@ -16,7 +17,7 @@
 #define ZH_BB 512              // threads of the binning kernel
 #define ZH_SMEM_BINS 4096      // bins up to this many use per-CTA shared-memory histograms (64 KB with weights)
 #define ZH_SB 256              // threads of the spline kernel
-#define ZH_K 3                 // spline degree
+#define ZH_K NBK_SPLEV_K       // spline degree
 
 // ---------------------------------------------------------------------------------------------------------------------
 // moments
@@ -196,40 +197,6 @@ __global__ void __launch_bounds__(ZH_BB) k_zh_bin(const T *__restrict__ z, const
 // ---------------------------------------------------------------------------------------------------------------------
 // spline
 
-// FITPACK splev for k = 3 at x: the knot interval l (t[l] <= x < t[l+1], clamped to [k, nt - k - 2]) and fpbspl
-static __device__ __forceinline__ double zh_splev(double x, const double *__restrict__ t, int nt, const double *__restrict__ c) {
-    int lo = ZH_K, hi = nt - ZH_K - 1;           // the largest l in [k, nt - k - 2] with t[l] <= x (k when none)
-    while (hi - lo > 1) {
-        const int mid = (lo + hi) >> 1;
-        if (__ldg(t + mid) <= x) lo = mid;
-        else hi = mid;
-    }
-    const int l = lo;
-    double h[ZH_K + 1], hh[ZH_K];
-    h[0] = 1.0;
-#pragma unroll
-    for (int j = 1; j <= ZH_K; j++) {
-#pragma unroll
-        for (int i = 0; i < j; i++) hh[i] = h[i];
-        h[0] = 0.0;
-#pragma unroll
-        for (int i = 1; i <= j; i++) {
-            const double tli = __ldg(t + l + i), tlj = __ldg(t + l + i - j);
-            if (tli == tlj) {
-                h[i] = 0.0;
-                continue;
-            }
-            const double f = hh[i - 1] / (tli - tlj);
-            h[i - 1] = h[i - 1] + f * (tli - x);
-            h[i] = f * (x - tlj);
-        }
-    }
-    double sp = 0.0;
-#pragma unroll
-    for (int j = 0; j <= ZH_K; j++) sp = sp + __ldg(c + l - ZH_K + j) * h[j];
-    return sp;
-}
-
 template <typename T>
 __global__ void __launch_bounds__(ZH_SB) k_zh_spline(const T *__restrict__ z, long long n, const double *__restrict__ t, int nt,
                                                      const double *__restrict__ c, int ext, double *__restrict__ out,
@@ -246,7 +213,7 @@ __global__ void __launch_bounds__(ZH_SB) k_zh_spline(const T *__restrict__ z, lo
             v = 0.0;
         } else {
             if (oob && ext == 3) x = x < tb ? tb : te;
-            v = zh_splev(x, t, nt, c);
+            v = nbk_splev3(x, t, nt, c);
         }
         out[i] = v;
     }

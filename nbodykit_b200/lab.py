@@ -7,4 +7,4 @@ from .source.mesh import *  # noqa: F401,F403
 from .algorithms import *  # noqa: F401,F403
 from .binned_statistic import BinnedStatistic  # noqa: F401
 from . import cosmology, transform  # noqa: F401
-from .hod import HODModel, Zheng07Model  # noqa: F401
+from .hod import HODModel, Hearin15Model, Leauthaud11Model, Zheng07Model  # noqa: F401

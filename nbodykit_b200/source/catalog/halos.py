@@ -1,12 +1,13 @@
 """
 HaloCatalog and PopulatedHaloCatalog (API of nbodykit/source/catalog/halos.py) on one or several GPUs.
 
-The reference hands each rank's halos to halotools on the CPU.  Here the Zheng07 model of :mod:`nbodykit_b200.hod` is
-evaluated by this package's kernels (csrc/hod.cu) to the contract of DESIGN.md 4.13: one occupation draw per halo, a
-scan for the galaxy rows, then one thread per galaxy for its position and velocity.  Every draw is a counter-based hash
-of (seed, stream, global halo row, draw index), so the catalogue is the same for any number of ranks and any split of
-the halo rows.  Galaxies stay on the rank of their halo: on every rank the centrals of its halos come first, in halo
-order, then the satellites, in (halo, satellite) order.
+The reference hands each rank's halos to halotools on the CPU.  Here the Zheng07, Leauthaud11 and Hearin15 models of
+:mod:`nbodykit_b200.hod` are evaluated by this package's kernels (csrc/hod.cu) to the contract of DESIGN.md 4.13: one
+occupation draw per halo, a scan for the galaxy rows, then one thread per galaxy for its position and velocity.
+Hearin15 also ranks each halo's secondary property among the halos of its mass bin on all ranks, once per catalogue.
+Every draw is a counter-based hash of (seed, stream, global halo row, draw index), so the catalogue is the same for any
+number of ranks and any split of the halo rows.  Galaxies stay on the rank of their halo: on every rank the centrals
+of its halos come first, in halo order, then the satellites, in (halo, satellite) order.
 """
 import logging
 import math
@@ -19,6 +20,7 @@ from ... import CurrentMPIComm
 from ... import transform
 from ..._lib import F4, F8, check, darr, lib, stage
 from ...base.catalog import CatalogSource, CatalogSourceBase, Column, ConstantColumn, column
+from ...base.ordering import global_rank, key_tensor
 from ...cosmology import Cosmology, G_KMS2_MPC_PER_MSUN
 from ...pmesh.pm import _ptr, _stream, as_device_tensor, current_device
 from .array import ArrayCatalog
@@ -125,7 +127,8 @@ class HaloCatalog(CatalogSource):
 
         Parameters
         ----------
-        model : :class:`~nbodykit_b200.hod.Zheng07Model` class or instance
+        model : :class:`~nbodykit_b200.hod.Zheng07Model`, :class:`~nbodykit_b200.hod.Leauthaud11Model` or
+            :class:`~nbodykit_b200.hod.Hearin15Model`, class or instance
             the occupation model
         BoxSize : float, 3-vector, optional
             the box the galaxy positions wrap into; ``attrs['BoxSize']`` when not given
@@ -143,20 +146,62 @@ class HaloCatalog(CatalogSource):
         model.check()
         box = _box(BoxSize if BoxSize is not None else self.attrs.get('BoxSize', None))
         seed = _seed(self.comm, seed)
-        halos = _Halos(self, box)
-        return PopulatedHaloCatalog._populate(halos, model, seed, self.cosmo, self.comm)
+        occ = _occupation(model, self.attrs['redshift'])
+        sec = _check_sec(self, model)
+        halos = _Halos(self, box, sec)
+        return PopulatedHaloCatalog._populate(halos, model, seed, self.cosmo, self.comm, occ)
 
 
 def _as_model(model):
-    from ...hod import HODModel, Zheng07Model
+    from ...hod import HODModel, Hearin15Model, Leauthaud11Model, Zheng07Model
     if isinstance(model, type) and issubclass(model, HODModel):
         model = model()
     if not isinstance(model, HODModel):
         raise TypeError("model for populating mocks should be an nbodykit_b200.hod.HODModel subclass (got %r)" % (model,))
-    if not isinstance(model, Zheng07Model):
-        raise NotImplementedError("only Zheng07Model is implemented (got %s)" % type(model).__name__)
-    # a private copy: populate and repopulate update its parameters
-    return Zheng07Model(modulate_with_cenocc=model.modulate_with_cenocc, **model.param_dict)
+    for cls in (Hearin15Model, Leauthaud11Model, Zheng07Model):
+        if isinstance(model, cls):
+            # a private copy: populate and repopulate update its parameters
+            return cls(**dict(model.arguments(), **model.param_dict))
+    raise NotImplementedError("only Zheng07Model, Leauthaud11Model and Hearin15Model are implemented (got %s)"
+                              % type(model).__name__)
+
+
+def _occupation(model, redshift):
+    """the host-side inputs of the occupation kernel (the SMHM spline of Leauthaud11 and Hearin15; None for Zheng07)"""
+    from ...hod import Leauthaud11Model
+    return model.occupation(redshift) if isinstance(model, Leauthaud11Model) else None
+
+
+def _check_sec(cat, model):
+    """the name of the Hearin15 secondary halo property (None for other models), after checking on all ranks that it is
+    a 1-D column of finite numbers"""
+    from ...hod import Hearin15Model
+    if not isinstance(model, Hearin15Model):
+        return None
+    name = model.sec_haloprop
+    if name not in cat:
+        raise ValueError("Hearin15Model: the halo catalogue has no sec_haloprop column '%s'" % name)
+    v = _values(cat[name])
+    shape = tuple(v.shape)
+    if isinstance(v, torch.Tensor):
+        nonfinite = int((~torch.isfinite(v)).sum().item()) if (v.is_floating_point() or v.is_complex()) else 0
+        numeric = v.is_floating_point() or v.dtype in (torch.int8, torch.uint8, torch.int16, torch.int32, torch.int64)
+    else:
+        v = numpy.asarray(v)
+        numeric = numpy.issubdtype(v.dtype, numpy.integer) or numpy.issubdtype(v.dtype, numpy.floating)
+        nonfinite = int((~numpy.isfinite(v)).sum()) if numeric else 0
+    bad_shape = int(_allreduce(cat.comm, int(len(shape) != 1 or not numeric)))
+    nonfinite = int(_allreduce(cat.comm, nonfinite))
+    if bad_shape:
+        raise ValueError("Hearin15Model: sec_haloprop '%s' must be a one-dimensional numeric column" % name)
+    if nonfinite:
+        raise ValueError("Hearin15Model: sec_haloprop '%s' has %d non-finite values" % (name, nonfinite))
+    return name
+
+
+def _allreduce(comm, x):
+    """the sum of x over the ranks"""
+    return comm.allreduce(x) if comm.size > 1 else x
 
 
 def _box(BoxSize):
@@ -185,10 +230,12 @@ def _values(col):
 
 
 class _Halos(object):
-    """the halo columns the kernels read, on the device, and this rank's first global halo row"""
+    """the halo columns the kernels read, on the device, and this rank's first global halo row; for Hearin15 the
+    secondary halo property `sec` and the percentiles of each halo in its mass bin, cached per (sec, bin width)"""
 
-    def __init__(self, cat, box):
+    def __init__(self, cat, box, sec=None):
         comm = cat.comm
+        self.comm = comm
         cols = {k: _values(cat[k]) for k in ('Mass', 'Radius', 'Concentration', 'Position', 'Velocity')}
         bad = 0
         for k in ('Mass', 'Radius', 'Concentration'):
@@ -229,18 +276,65 @@ class _Halos(object):
         self.rsd = (1 + z) / (100. * cat.cosmo.efunc(z))
         from ...hod import jeans_table
         self.table = torch.from_numpy(jeans_table()).to(dev)
+        self.sec = {}
+        if sec is not None:
+            self.sec[sec] = key_tensor(cat[sec], sec, device=dev)
+        self._pct = {}
 
-    def run(self, model, seed):
-        """the galaxy columns of (model, seed) on this rank, and the local numbers of centrals and galaxies"""
-        from ...hod import JEANS_HS, JEANS_K, JEANS_S0
+    def percentiles(self, sec, d):
+        """float64 (n,): (rank + 1) / N_bin of each halo among the N_bin halos of all ranks in its mass bin
+        floor(log10 M / d), ranked by (sec, global row)"""
+        key = (sec, d)
+        if key not in self._pct:
+            comm, n = self.comm, self.n
+            with stage("hod_percentile"):
+                b = torch.floor(torch.log10(self.mass) / d)
+                lo = float(b.min().item()) if n else math.inf
+                hi = float(b.max().item()) if n else -math.inf
+                if comm.size > 1:
+                    lo, hi = float(comm.allreduce(lo, "min")), float(comm.allreduce(hi, "max"))
+                nb = hi - lo + 1
+                if not nb <= (1 << 24):
+                    raise ValueError("Hearin15Model: %g mass bins of width dlog10_prim_haloprop = %r; at most 2^24"
+                                     % (nb, d))
+                bins = (b - lo).to(torch.int64)
+                pos = global_rank(comm, [bins, self.sec[sec]], n, self.mass.device)
+                cnt = torch.bincount(bins, minlength=int(nb)) if n else \
+                    torch.zeros(int(nb), dtype=torch.int64, device=self.mass.device)
+                if comm.size > 1:
+                    comm.allreduce_tensor(cnt, "sum")
+                start = torch.cumsum(cnt, 0) - cnt
+                self._pct[key] = ((pos - start[bins] + 1).to(torch.float64) / cnt[bins].to(torch.float64)).contiguous()
+        return self._pct[key]
+
+    def run(self, model, seed, occ=None):
+        """the galaxy columns of (model, seed) on this rank, and the local numbers of centrals and galaxies; `occ` holds
+        the host-side inputs of the SMHM occupation (Leauthaud11, Hearin15)"""
+        from ...hod import JEANS_HS, JEANS_K, JEANS_S0, Hearin15Model
         n, dev = self.n, self.pos.device
         p = model.param_dict
         L = lib()
         counts = torch.empty(2 * n, dtype=torch.int64, device=dev)
-        with stage("hod_occupy"):
-            check(L.nbk_hod_occupy(_ptr(self.mass), F8, n, self.h0, p['logMmin'], p['sigma_logM'], 10. ** p['logM0'],
-                                   10. ** p['logM1'], p['alpha'], int(model.modulate_with_cenocc), seed, _ptr(counts),
-                                   _stream()), "nbk_hod_occupy")
+        if occ is None:
+            with stage("hod_occupy"):
+                check(L.nbk_hod_occupy(_ptr(self.mass), F8, n, self.h0, p['logMmin'], p['sigma_logM'],
+                                       10. ** p['logM0'], 10. ** p['logM1'], p['alpha'],
+                                       int(model.modulate_with_cenocc), seed, _ptr(counts), _stream()),
+                      "nbk_hod_occupy")
+        else:
+            pct, split, acen, asat = None, 0.5, 0.0, 0.0
+            if isinstance(model, Hearin15Model):
+                pct = self.percentiles(model.sec_haloprop, model.dlog10_prim_haloprop)
+                split = model.split
+                acen, asat = model.strengths()
+            tc = torch.from_numpy(numpy.concatenate([occ['t'], occ['c']])).to(dev)
+            nt = occ['t'].size
+            with stage("hod_occupy"):
+                check(L.nbk_hod_occupy_smhm(_ptr(self.mass), F8, n, self.h0, _ptr(tc), nt, _ptr(tc[nt:]),
+                                            model.threshold, p['scatter_model_param1'], occ['Msat'], occ['Mcut'],
+                                            p['alphasat'], int(model.modulate_with_cenocc),
+                                            _ptr(pct), split, acen, asat, seed,
+                                            _ptr(counts), _stream()), "nbk_hod_occupy_smhm")
         with stage("hod_scan"):
             offsets = torch.empty(2 * n + 1, dtype=torch.int64, device=dev)
             wb = int(L.nbk_hod_scan_workspace(2 * n))
@@ -288,8 +382,8 @@ class PopulatedHaloCatalog(ArrayCatalog):
         self.cosmo = cosmo
 
     @classmethod
-    def _populate(cls, halos, model, seed, cosmo, comm, into=None):
-        data, ncen, ngal = halos.run(model, seed)
+    def _populate(cls, halos, model, seed, cosmo, comm, occ=None, into=None):
+        data, ncen, ngal = halos.run(model, seed, occ)
         if into is None:
             into = cls.__new__(cls)
         else:
@@ -304,7 +398,7 @@ class PopulatedHaloCatalog(ArrayCatalog):
         nsat = int(comm.allreduce(ngal - ncen))
         into.attrs.update(halos.attrs)
         into.attrs.update(model.param_dict)
-        into.attrs['modulate_with_cenocc'] = model.modulate_with_cenocc
+        into.attrs.update(model.arguments())
         into.attrs['seed'] = seed
         into.attrs['gal_types'] = {t: i for i, t in enumerate(model.gal_types)}
         into.attrs['fsat'] = float(nsat) / into.csize
@@ -319,4 +413,5 @@ class PopulatedHaloCatalog(ArrayCatalog):
         model.update(params)
         model.check()
         seed = _seed(self.comm, seed)
-        PopulatedHaloCatalog._populate(self._halos, model, seed, self.cosmo, self.comm, into=self)
+        occ = _occupation(model, self._halos.attrs['redshift'])
+        PopulatedHaloCatalog._populate(self._halos, model, seed, self.cosmo, self.comm, occ, into=self)
