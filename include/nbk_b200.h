@@ -177,7 +177,11 @@ int nbk_fft_z_bluestein(const void *in, void *out, int dtype, int64_t rows, int6
  *   pack    : cplx slab [x_n][Ny][Nzc] -> send buffer [P][y_n][x_n][Nzc] (block p = y rows of rank p)
  *   x pass  : after the all-to-all the receive buffer [P][y_n][x_n][Nzc] IS [y_n][Nx][Nzc] re-ordered;
  *             unpack -> [y_n][Nx][Nzc], FFT along x, scale by `scale`.
- * and their inverses for c2r. */
+ * and their inverses for c2r.
+ * nbk_fft_zy_forward (and so nbk_r2c) runs the z and y passes as one pipelined kernel for f8 fields with Nz and Ny in
+ * {256, 512, 1024} whose slab is larger than half the L2 (DESIGN 4.2).  Its CTAs coordinate through a ticket counter and progress flags owned by the calling stream:
+ * calls on different streams may run concurrently, calls on one stream run in order.  It is not meant for capture into
+ * a CUDA graph (a replay would reuse the captured call's flags). */
 int nbk_fft_zy_forward(const void *real, void *cplx, int dtype, int64_t x_n, int64_t Ny, int64_t Nz,
                        void *stream);
 int nbk_fft_zy_backward(void *cplx, void *real, int dtype, int64_t x_n, int64_t Ny, int64_t Nz,

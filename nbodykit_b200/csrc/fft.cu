@@ -14,6 +14,8 @@
 //   k_fft_lines_tma   lines of 256 / 512 / 1024: row groups stream through a ring of shared-memory slots as 4-D tensor-map
 //                     boxes (cp.async.bulk.tensor + mbarrier), one 64-point FFT per warp, one radix-R combine per tile
 //   k_fft_z_r2c_tma   rows of 256 / 512 / 1024 reals: warp-per-row, private ring of row buffers filled by 1-D bulk copies
+//   k_fft_zy_r2c_pipe the forward z and y passes of c16 fields where both of the above apply, pipelined plane by plane
+//                     so that the y tiles read the z rows from L2 (same device functions, same bits)
 // Older families, still serving the other lengths, c8 lines whose rows are not 16-byte aligned and the backward z pass:
 // the register-I/O kernels for lines of 64 and more (k_fft_lines_rg, k_fft_z_r2c_rg: first radix-8 stage straight from
 // global memory, last stage straight to the digit-reversed frequency rows, [N][B+1] padded tiles in between) and the
@@ -648,6 +650,88 @@ template <int R, typename C> __device__ __forceinline__ void dftR(C (&a)[R]) {
 // the whole SM).  Also its launch bound: without it ptxas trades spills for an occupancy the ring rules out.
 __host__ __device__ constexpr int tma_ctas_per_sm(int R) { return R == 16 ? 1 : R == 4 ? 3 : 2; }
 
+// One tile of the TMA line pass: its R row groups are landing in the ring slots (g0 + j) % NS (g0 = groups this CTA
+// streamed before the tile, which also gives each slot's mbarrier phase).  The NT threads run the 64-point FFTs (warp
+// w owns groups w, w + NW, ...; warps beyond R wait), the radix-R combine and the stores, then free the R slots: on
+// return they may be refilled.
+template <typename T, int R, int B, int NT, bool PEER>
+__device__ __forceinline__ void lines_tma_tile(typename C2<T>::type *ring, uint64_t *bars, int NS, int g0,
+                                               const typename C2<T>::type *twN, const typename C2<T>::type *tw64,
+                                               typename C2<T>::type *dst, const PeerPtrs<typename C2<T>::type> &peers,
+                                               int64_t line_stride, int64_t n_inner, int64_t outer_stride, int n_per,
+                                               int64_t d_total, int64_t outer_start, int64_t outer, int64_t inner0,
+                                               T sgn, T scale) {
+    typedef typename C2<T>::type C;
+    constexpr int S = 64, NW = NT / 32, SLOT = S * B;
+    static_assert((8 * B) % 32 == 0 && (R % NW == 0 || NW % R == 0), "tile geometry");
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int bvalid = (int)((n_inner - inner0) < B ? (n_inner - inner0) : B);
+    // ---- 64-point FFT of my row group (warp-local: two radix-8 stages in place)
+    for (int gw = warp; gw < R; gw += NW) {
+        const int g = g0 + gw, slot = g % NS;
+        fm_mbar_wait(&bars[slot], (unsigned)((g / NS) & 1));
+        C *sl = ring + (size_t)slot * SLOT;
+        constexpr int IT = (8 * B) / 32;
+#pragma unroll
+        for (int i = 0; i < IT; i++) {
+            const int w = lane + 32 * i, b = w % B, q = w / B;
+            C *p = sl + q * B + b;
+            C a[8];
+#pragma unroll
+            for (int j = 0; j < 8; j++) { a[j] = p[j * 8 * B]; a[j].y *= sgn; }
+            radix8(a);
+            p[0] = a[0];
+#pragma unroll
+            for (int m = 1; m < 8; m++) p[m * 8 * B] = cmul(a[m], tw64[m * q]);
+        }
+        __syncwarp();
+#pragma unroll
+        for (int i = 0; i < IT; i++) {
+            const int w = lane + 32 * i, b = w % B, t = w / B;
+            C *p = sl + t * 8 * B + b;
+            C a[8];
+#pragma unroll
+            for (int j = 0; j < 8; j++) a[j] = p[j * B];
+            radix8(a);
+#pragma unroll
+            for (int m = 0; m < 8; m++) p[m * B] = a[m];       // position 8 t + m holds frequency t + 8 m
+        }
+    }
+    __syncthreads();
+    // ---- radix-R combine across the groups, registers -> global frequency rows k + 64 m
+    {
+        const int base = g0 % NS;
+        for (int w = tid; w < S * B; w += NT) {
+            const int b = w % B, k = w / B;
+            const int pos = ((k & 7) << 3) | (k >> 3);
+            C a[R];
+#pragma unroll
+            for (int j = 0; j < R; j++) {
+                int sj = base + j;
+                if (sj >= NS) sj -= NS;
+                C v = ring[(size_t)sj * SLOT + pos * B + b];
+                a[j] = j ? cmul(v, twN[j * k]) : v;
+            }
+            dftR<R, C>(a);
+            if (b < bvalid) {
+#pragma unroll
+                for (int m = 0; m < R; m++) {
+                    const int K = k + S * m;
+                    const C v = C{a[m].x * scale, a[m].y * sgn * scale};
+                    if (PEER) {
+                        const int pr = K / n_per, kl = K - pr * n_per;
+                        peers.p[pr][((int64_t)kl * d_total + outer_start + outer) * n_inner + inner0 + b] = v;
+                    } else {
+                        dst[outer * outer_stride + inner0 + (int64_t)K * line_stride + b] = v;
+                    }
+                }
+            }
+        }
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic accesses to the slots before the next TMA writes
+    __syncthreads();
+}
+
 template <typename T, int R, int B, int NT, bool PEER>
 __global__ void __launch_bounds__(NT, tma_ctas_per_sm(R))
 k_fft_lines_tma(const __grid_constant__ CUtensorMap tmap, typename C2<T>::type *dst, PeerPtrs<typename C2<T>::type> peers,
@@ -656,14 +740,14 @@ k_fft_lines_tma(const __grid_constant__ CUtensorMap tmap, typename C2<T>::type *
                 int NS) {
     typedef typename C2<T>::type C;
     // B side-by-side lines: 128-byte rows (8 c16 / 16 c8)
-    constexpr int S = 64, N = S * R, NW = NT / 32, SLOT = S * B;
-    static_assert((8 * B) % 32 == 0 && R % NW == 0, "tile geometry");
+    constexpr int S = 64, N = S * R, SLOT = S * B;
+    static_assert(R % (NT / 32) == 0, "tile geometry");
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     C *ring = reinterpret_cast<C *>(smem_raw);                 // [NS][64][B]
     C *twN = ring + (size_t)NS * SLOT;                         // W_N^i, i < N
     C *tw64 = twN + N;                                         // W_64^i, i < 64
     uint64_t *bars = reinterpret_cast<uint64_t *>(tw64 + S);   // [NS]
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int tid = threadIdx.x;
     if (tid == 0) {
         for (int i = 0; i < NS; i++) fm_mbar_init(&bars[i], 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -693,71 +777,8 @@ k_fft_lines_tma(const __grid_constant__ CUtensorMap tmap, typename C2<T>::type *
         const int64_t tile = first + (int64_t)it * gridDim.x;
         const int64_t outer = tile / tiles_inner;
         const int64_t inner0 = (tile - outer * tiles_inner) * B;
-        const int bvalid = (int)((n_inner - inner0) < B ? (n_inner - inner0) : B);
-        // ---- 64-point FFT of my row group (warp-local: two radix-8 stages in place)
-        for (int gw = warp; gw < R; gw += NW) {
-            const int g = it * R + gw, slot = g % NS;
-            fm_mbar_wait(&bars[slot], (unsigned)((g / NS) & 1));
-            C *sl = ring + (size_t)slot * SLOT;
-            constexpr int IT = (8 * B) / 32;
-#pragma unroll
-            for (int i = 0; i < IT; i++) {
-                const int w = lane + 32 * i, b = w % B, q = w / B;
-                C *p = sl + q * B + b;
-                C a[8];
-#pragma unroll
-                for (int j = 0; j < 8; j++) { a[j] = p[j * 8 * B]; a[j].y *= sgn; }
-                radix8(a);
-                p[0] = a[0];
-#pragma unroll
-                for (int m = 1; m < 8; m++) p[m * 8 * B] = cmul(a[m], tw64[m * q]);
-            }
-            __syncwarp();
-#pragma unroll
-            for (int i = 0; i < IT; i++) {
-                const int w = lane + 32 * i, b = w % B, t = w / B;
-                C *p = sl + t * 8 * B + b;
-                C a[8];
-#pragma unroll
-                for (int j = 0; j < 8; j++) a[j] = p[j * B];
-                radix8(a);
-#pragma unroll
-                for (int m = 0; m < 8; m++) p[m * B] = a[m];       // position 8 t + m holds frequency t + 8 m
-            }
-        }
-        __syncthreads();
-        // ---- radix-R combine across the groups, registers -> global frequency rows k + 64 m
-        {
-            const int base = (it * R) % NS;
-            for (int w = tid; w < S * B; w += NT) {
-                const int b = w % B, k = w / B;
-                const int pos = ((k & 7) << 3) | (k >> 3);
-                C a[R];
-#pragma unroll
-                for (int j = 0; j < R; j++) {
-                    int sj = base + j;
-                    if (sj >= NS) sj -= NS;
-                    C v = ring[(size_t)sj * SLOT + pos * B + b];
-                    a[j] = j ? cmul(v, twN[j * k]) : v;
-                }
-                dftR<R, C>(a);
-                if (b < bvalid) {
-#pragma unroll
-                    for (int m = 0; m < R; m++) {
-                        const int K = k + S * m;
-                        const C v = C{a[m].x * scale, a[m].y * sgn * scale};
-                        if (PEER) {
-                            const int pr = K / n_per, kl = K - pr * n_per;
-                            peers.p[pr][((int64_t)kl * d_total + outer_start + outer) * n_inner + inner0 + b] = v;
-                        } else {
-                            dst[outer * outer_stride + inner0 + (int64_t)K * line_stride + b] = v;
-                        }
-                    }
-                }
-            }
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic accesses to the slots before the next TMA writes
-        __syncthreads();
+        lines_tma_tile<T, R, B, NT, PEER>(ring, bars, NS, it * R, twN, tw64, dst, peers, line_stride, n_inner,
+                                          outer_stride, n_per, d_total, outer_start, outer, inner0, sgn, scale);
         if (tid == 0) {
             int upto = (it + 1) * R + NS;
             if (upto > G) upto = G;
@@ -992,47 +1013,77 @@ __device__ __forceinline__ void fm_bulk_g2s(void *sdst, const void *gsrc, unsign
 }
 __device__ __forceinline__ int fm_sw(int e) { return e ^ ((e >> 3) & 7); }
 
-template <typename T, int LM, int NW>
-__global__ void __launch_bounds__(32 * NW)
-k_fft_z_r2c_tma(const T *__restrict__ real, typename C2<T>::type *__restrict__ cplx,
-                const typename C2<T>::type *__restrict__ twN_g, int64_t rows, T scale, int nbuf) {
+// L2 policies for the pipelined z + y pass (k_fft_zy_r2c_pipe): its z stores ask L2 to keep their lines for the y
+// tiles that read them back, and its reads of the real field, used once, ask to leave first.
+__device__ __forceinline__ uint64_t l2_policy_evict_last() {
+    uint64_t p;
+    asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+__device__ __forceinline__ uint64_t l2_policy_evict_first() {
+    uint64_t p;
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+__device__ __forceinline__ void st_hint(double2 *p, double2 v, uint64_t pol) {
+    asm volatile("st.global.L2::cache_hint.v2.f64 [%0], {%1, %2}, %3;" :: "l"(p), "d"(v.x), "d"(v.y), "l"(pol) : "memory");
+}
+__device__ __forceinline__ void st_hint(float2 *p, float2 v, uint64_t pol) {
+    asm volatile("st.global.L2::cache_hint.v2.f32 [%0], {%1, %2}, %3;" :: "l"(p), "f"(v.x), "f"(v.y), "l"(pol) : "memory");
+}
+__device__ __forceinline__ void fm_bulk_g2s_hint(void *sdst, const void *gsrc, unsigned bytes, uint64_t *bar, uint64_t pol) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
+                 :: "r"(fm_smem_u32(sdst)), "l"(gsrc), "r"(bytes), "r"(fm_smem_u32(bar)), "l"(pol) : "memory");
+}
+
+// Twiddle tables of the warp-per-row z pass in shared memory: W_N^i, i < Nz (Hermitian split) | [7][Q1] W_M^{q m},
+// lanes along q at unit stride | [7][8] W_{8 R3}^{q m}.  All threads of the CTA call; a CTA barrier must follow.
+template <typename C, int LM, int NT>
+__device__ __forceinline__ void z_r2c_stage_twiddles(C *twN, const C *__restrict__ twN_g) {
+    constexpr int M = 1 << LM, Nz = 2 * M, R3 = M / 64, Q1 = M / 8;
+    C *tw1 = twN + Nz, *tw2 = tw1 + 7 * Q1;
+    for (int i = threadIdx.x; i < Nz; i += NT) twN[i] = twN_g[i];
+    // (a strided twN[2 m q] / twN[16 m q] puts the lanes of a quarter warp on the same banks: 8-way conflicts that made
+    // the twiddle reads cost more shared-memory wavefronts than the data)
+    for (int i = threadIdx.x; i < 7 * Q1; i += NT) { const int m = i / Q1 + 1, q = i % Q1; tw1[i] = twN_g[2 * m * q]; }
+    for (int i = threadIdx.x; i < 7 * R3; i += NT) { const int m = i / R3 + 1, q = i % R3; tw2[i] = twN_g[(16 * m * q) % Nz]; }
+}
+template <int LM> __host__ __device__ constexpr int z_r2c_twiddle_len() { return 2 * (1 << LM) + 7 * ((1 << LM) / 8) + 7 * 8; }
+
+// One warp transforms n real rows, row i = first + i * stride (i < n), streaming them through its private ring of nbuf
+// row buffers (wbuf [nbuf][M], one mbarrier each in wbar).  c0 = rows the warp streamed through the ring before: slots
+// and mbarrier phases continue from there.  KEEP: the real rows are read with an L2 evict-first hint and the complex
+// rows stored with an evict-last one (the pipelined z + y pass); otherwise plain loads and stores.
+template <typename T, int LM, bool KEEP>
+__device__ __forceinline__ void z_r2c_warp_rows(const T *__restrict__ real, typename C2<T>::type *__restrict__ cplx,
+                                                const typename C2<T>::type *twN, typename C2<T>::type *wbuf,
+                                                uint64_t *wbar, int nbuf, int64_t c0, int64_t first, int64_t stride,
+                                                int64_t n, T h) {
     typedef typename C2<T>::type C;
     constexpr int M = 1 << LM, Nz = 2 * M, Nzc = M + 1;
     constexpr int R3 = M / 64;                    // last radix: 8 / 4 / 2
     constexpr int Q1 = M / 8;                     // butterflies of the radix-8 stages
     constexpr int I1 = (Q1 + 31) / 32;            // ... per lane
-    extern __shared__ __align__(128) unsigned char smem_raw[];
-    C *twN = reinterpret_cast<C *>(smem_raw);                         // W_N^i, i <= M  (Hermitian split)
-    C *tw1 = twN + Nz;                                                // [7][Q1]  W_M^{q m}: lanes along q, unit stride
-    C *tw2 = tw1 + 7 * Q1;                                            // [7][R3]  W_{8 R3}^{q m}
-    C *bufs = tw2 + 7 * 8;                                            // [NW][nbuf][M]
-    uint64_t *bars = reinterpret_cast<uint64_t *>(bufs + (size_t)NW * nbuf * M);   // [NW][nbuf]
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    for (int i = threadIdx.x; i < Nz; i += 32 * NW) twN[i] = twN_g[i];
-    // (a strided twN[2 m q] / twN[16 m q] puts the lanes of a quarter warp on the same banks: 8-way conflicts that made
-    // the twiddle reads cost more shared-memory wavefronts than the data)
-    for (int i = threadIdx.x; i < 7 * Q1; i += 32 * NW) { const int m = i / Q1 + 1, q = i % Q1; tw1[i] = twN_g[2 * m * q]; }
-    for (int i = threadIdx.x; i < 7 * R3; i += 32 * NW) { const int m = i / R3 + 1, q = i % R3; tw2[i] = twN_g[(16 * m * q) % Nz]; }
-    if (lane == 0) {
-        for (int i = 0; i < nbuf; i++) fm_mbar_init(&bars[warp * nbuf + i], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-    const int64_t gw = (int64_t)blockIdx.x * NW + warp, GW = (int64_t)gridDim.x * NW;
-    const int64_t my_rows = gw < rows ? (rows - gw + GW - 1) / GW : 0;
-    C *wbuf = bufs + (size_t)warp * nbuf * M;
-    uint64_t *wbar = bars + warp * nbuf;
+    const C *tw1 = twN + Nz, *tw2 = tw1 + 7 * Q1;
+    // read here (volatile): in the persistent k_fft_zy_r2c_pipe the per-lane shared addresses would otherwise be hoisted
+    // out of its work loop, held across the y tiles, and spilled
+    int lane;
+    asm volatile("mov.u32 %0, %%laneid;" : "=r"(lane));
+    lane &= 31;
     const unsigned row_bytes = (unsigned)(M * sizeof(C));
+    uint64_t pol_in = 0, pol_out = 0;
+    if (KEEP) { pol_in = l2_policy_evict_first(); pol_out = l2_policy_evict_last(); }
     auto issue = [&](int64_t i) {     // lane 0 only
-        const int sidx = (int)(i % nbuf);
+        const int sidx = (int)((c0 + i) % nbuf);
         fm_mbar_expect_tx(&wbar[sidx], row_bytes);
-        fm_bulk_g2s(wbuf + (size_t)sidx * M, real + (gw + i * GW) * (int64_t)Nz, row_bytes, &wbar[sidx]);
+        const T *src = real + (first + i * stride) * (int64_t)Nz;
+        if (KEEP) fm_bulk_g2s_hint(wbuf + (size_t)sidx * M, src, row_bytes, &wbar[sidx], pol_in);
+        else fm_bulk_g2s(wbuf + (size_t)sidx * M, src, row_bytes, &wbar[sidx]);
     };
-    if (lane == 0) for (int64_t i = 0; i < nbuf && i < my_rows; i++) issue(i);
-    const T h = (T)0.5 * scale;
-    for (int64_t i = 0; i < my_rows; i++) {
-        const int sidx = (int)(i % nbuf);
-        fm_mbar_wait(&wbar[sidx], (unsigned)((i / nbuf) & 1));
+    if (lane == 0) for (int64_t i = 0; i < nbuf && i < n; i++) issue(i);
+    for (int64_t i = 0; i < n; i++) {
+        const int sidx = (int)((c0 + i) % nbuf);
+        fm_mbar_wait(&wbar[sidx], (unsigned)(((c0 + i) / nbuf) & 1));
         C *z = wbuf + (size_t)sidx * M;
         // ---- stage 1 (radix 8 over elements q + Q1 j): reads the landed (unswizzled) row, writes swizzled
         {
@@ -1099,18 +1150,161 @@ k_fft_z_r2c_tma(const T *__restrict__ real, typename C2<T>::type *__restrict__ c
         }
         __syncwarp();
         // ---- Hermitian split, lanes along k:  X[k] = 1/2 [ (Z[k] + conj Z[M-k]) - i W_N^k (Z[k] - conj Z[M-k]) ]
-        C *drow = cplx + (gw + i * GW) * (int64_t)Nzc;
+        C *drow = cplx + (first + i * stride) * (int64_t)Nzc;
         for (int k = lane; k < Nzc; k += 32) {
             const C zk = z[fm_sw(k & (M - 1))];
             const C zm = cconj(z[fm_sw((M - k) & (M - 1))]);
             const C e = cadd(zk, zm), o = csub(zk, zm);
             const C wo = cmul(twN[k], o);
-            drow[k] = C{(e.x + wo.y) * h, (e.y - wo.x) * h};
+            const C v = C{(e.x + wo.y) * h, (e.y - wo.x) * h};
+            if (KEEP) st_hint(drow + k, v, pol_out);
+            else drow[k] = v;
         }
         // ---- the buffer is free: fetch the row that will use it next
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         __syncwarp();
-        if (lane == 0 && i + nbuf < my_rows) issue(i + nbuf);
+        if (lane == 0 && i + nbuf < n) issue(i + nbuf);
+    }
+}
+
+template <typename T, int LM, int NW>
+__global__ void __launch_bounds__(32 * NW)
+k_fft_z_r2c_tma(const T *__restrict__ real, typename C2<T>::type *__restrict__ cplx,
+                const typename C2<T>::type *__restrict__ twN_g, int64_t rows, T scale, int nbuf) {
+    typedef typename C2<T>::type C;
+    constexpr int M = 1 << LM;
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    C *twN = reinterpret_cast<C *>(smem_raw);                         // twiddle tables (z_r2c_stage_twiddles)
+    C *bufs = twN + z_r2c_twiddle_len<LM>();                          // [NW][nbuf][M]
+    uint64_t *bars = reinterpret_cast<uint64_t *>(bufs + (size_t)NW * nbuf * M);   // [NW][nbuf]
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    z_r2c_stage_twiddles<C, LM, 32 * NW>(twN, twN_g);
+    if (lane == 0) {
+        for (int i = 0; i < nbuf; i++) fm_mbar_init(&bars[warp * nbuf + i], 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    const int64_t gw = (int64_t)blockIdx.x * NW + warp, GW = (int64_t)gridDim.x * NW;
+    const int64_t my_rows = gw < rows ? (rows - gw + GW - 1) / GW : 0;
+    z_r2c_warp_rows<T, LM, false>(real, cplx, twN, bufs + (size_t)warp * nbuf * M, bars + warp * nbuf, nbuf, 0, gw, GW,
+                                  my_rows, (T)0.5 * scale);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Forward z + y passes of the power-of-two r2c, pipelined plane by plane (Nz = 2M, M in {128, 256, 512}; Ny = 64 R,
+// R in {4, 8, 16}; c16 fields).  Run one after the other, the z pass writes the whole half spectrum to HBM and the y
+// pass reads it straight back.  Here the y tiles of an x plane run shortly after that plane's z rows, so they read the
+// rows from L2, and their in-place stores overwrite lines that are still dirty there: each complex plane reaches DRAM
+// once (4 field-sizes of DRAM traffic for the r2c instead of 6).  The arithmetic is that of the two separate passes
+// (the same device functions, k_fft_z_r2c_tma's rows and k_fft_lines_tma's tiles): the result is bit-identical.
+//   * persistent CTAs of 512 threads take tickets from one global counter.  Ticket t is item t % L of step t / L, where
+//     a step lists the NZI z items of plane t / L (ZROWS rows each, warp-per-row) and then the NYI y tiles of plane
+//     t / L - D (B columns over all Ny rows); items of planes outside [0, x_n) are skipped;
+//   * a z item stamps its flag with this call's epoch once its rows are stored; a y tile polls the NZI flags of its
+//     plane (relaxed loads, then an acquire fence) and sleeps while any is older than the epoch;
+//   * deadlock-free by construction: a y tile waits only on z items of lower tickets, every one of which has been
+//     taken by a running CTA that never waits (z items wait on nothing), so the lowest unfinished ticket always makes
+//     progress -- whatever the grid size and however many CTAs are resident;
+//   * the ticket counter returns to 0 at the end of every call: every CTA takes tickets until one is past the last item,
+//     so exactly n_items + gridDim.x tickets are taken, and the CTA that takes the last one resets the counter.  The
+//     counter and the flags belong to the calling stream (ZyPipeSync): calls on other streams never touch them;
+//   * z and y items share the dynamic shared memory (z row buffers | y ring slots); each item drains its own copies
+//     before it returns, so the next item, of either kind, starts on free buffers.
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ unsigned ld_relaxed_gpu(const unsigned *p) {
+    unsigned v;
+    asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ void st_release_gpu(unsigned *p, unsigned v) {
+    asm volatile("st.release.gpu.global.u32 [%0], %1;" :: "l"(p), "r"(v) : "memory");
+}
+
+// threads of the pipelined z + y pass; rows per warp in one z item; complex values of each warp's z ring (its nbuf =
+// ZY_ZBUF / M row buffers: 1 / 2 / 4 at M = 512 / 256 / 128 fill the 128 KB a y tile of 1024-point lines takes)
+constexpr int ZY_NT = 512, ZY_ZPW = 2, ZY_ZBUF = 512;
+
+template <typename T, int LM, int R>
+__global__ void __launch_bounds__(ZY_NT, 1)
+k_fft_zy_r2c_pipe(const __grid_constant__ CUtensorMap tmap, const T *__restrict__ real, typename C2<T>::type *cplx,
+                  const typename C2<T>::type *__restrict__ twz_g, const typename C2<T>::type *__restrict__ twy_g,
+                  int x_n, int D, unsigned *ticket, unsigned *flags, unsigned epoch, T scale, T sgn) {
+    typedef typename C2<T>::type C;
+    constexpr int NT = ZY_NT, NW = NT / 32, M = 1 << LM, Nzc = M + 1, S = 64, Ny = S * R;
+    constexpr int B = 128 / (int)sizeof(C), SLOT = S * B;
+    constexpr int ZROWS = NW * ZY_ZPW;
+    constexpr int NZI = Ny / ZROWS, NYI = (Nzc + B - 1) / B, L = NZI + NYI;
+    constexpr int nbuf = ZY_ZBUF / M, NS = R;                // z ring: ZY_ZBUF complex per warp; y ring: one tile
+    static_assert(NZI <= 32, "one lane polls one z flag");
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    constexpr size_t zbuf = (size_t)NW * nbuf * M, ybuf = (size_t)NS * SLOT;
+    C *ring = reinterpret_cast<C *>(smem_raw);                 // z row buffers [NW][nbuf][M] | y slots [NS][64][B]
+    C *twz = ring + (zbuf > ybuf ? zbuf : ybuf);                // z twiddle tables (z_r2c_stage_twiddles)
+    C *twy = twz + z_r2c_twiddle_len<LM>();                    // W_Ny^i, i < Ny
+    C *tw64 = twy + Ny;                                        // W_64^i, i < 64
+    uint64_t *zbars = reinterpret_cast<uint64_t *>(tw64 + S);  // [NW][nbuf]
+    uint64_t *ybars = zbars + NW * nbuf;                       // [NS]
+    unsigned *s_ticket = reinterpret_cast<unsigned *>(ybars + NS);
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    z_r2c_stage_twiddles<C, LM, NT>(twz, twz_g);
+    for (int i = tid; i < Ny; i += NT) twy[i] = twy_g[i];
+    for (int i = tid; i < S; i += NT) tw64[i] = twy_g[i * R];
+    if (tid == 0) {
+        for (int i = 0; i < NW * nbuf; i++) fm_mbar_init(&zbars[i], 1);
+        for (int i = 0; i < NS; i++) fm_mbar_init(&ybars[i], 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    const PeerPtrs<C> no_peers{};
+    const unsigned n_items = (unsigned)L * (unsigned)(x_n + D);
+    const T h = (T)0.5 * scale;
+    int zc = 0;                 // rows each warp has streamed through its z ring
+    int yc = 0;                 // row groups the CTA has streamed through the y ring
+    for (;;) {
+        if (tid == 0) {
+            const unsigned t = atomicAdd(ticket, 1u);
+            if (t == n_items + gridDim.x - 1) atomicExch(ticket, 0u);
+            *s_ticket = t;
+        }
+        __syncthreads();
+        const unsigned t = *s_ticket;
+        __syncthreads();
+        if (t >= n_items) break;
+        const int step = (int)(t / L), r = (int)(t % L);
+        if (r < NZI) {
+            const int p = step;
+            if (p >= x_n) continue;
+            const int64_t row0 = (int64_t)p * Ny + (int64_t)r * ZROWS;
+            z_r2c_warp_rows<T, LM, true>(real, cplx, twz, ring + (size_t)warp * nbuf * M, zbars + warp * nbuf, nbuf, zc,
+                                         row0 + warp, NW, ZY_ZPW, h);
+            zc += ZY_ZPW;
+            asm volatile("fence.proxy.async.global;" ::: "memory");   // the rows are read back through the copy engine
+            __syncthreads();
+            if (tid == 0) st_release_gpu(&flags[(int64_t)p * NZI + r], epoch);   // cumulative over the CTA's stores
+        } else {
+            const int q = step - D;
+            if (q < 0) continue;
+            const int64_t inner0 = (int64_t)(r - NZI) * B;
+            if (warp == 0) {
+                if (lane < NZI) {
+                    const unsigned *f = flags + (int64_t)q * NZI + lane;
+                    while (ld_relaxed_gpu(f) < epoch) __nanosleep(256);
+                    asm volatile("fence.acq_rel.gpu;" ::: "memory");
+                }
+                __syncwarp();
+                if (lane == 0) {
+                    asm volatile("fence.proxy.async.global;" ::: "memory");
+                    for (int j = 0; j < R; j++) {
+                        const int slot = (yc + j) % NS;
+                        fm_mbar_expect_tx(&ybars[slot], (unsigned)(SLOT * sizeof(C)));
+                        fm_tma_load_4d(ring + (size_t)slot * SLOT, &tmap, (int)(2 * inner0), j, 0, q, &ybars[slot]);
+                    }
+                }
+            }
+            lines_tma_tile<T, R, B, NT, false>(ring, ybars, NS, yc, twy, tw64, cplx, no_peers, Nzc, Nzc,
+                                               (int64_t)Ny * Nzc, Ny, 0, 0, q, inner0, sgn, scale);
+            yc += R;
+        }
     }
 }
 
@@ -1225,6 +1419,34 @@ static int pick_B(int N, int csize, int64_t n_inner) {
 // TMA-pipelined line pass (k_fft_lines_tma) where it applies: N in {256, 512, 1024}, 16-byte aligned rows (always true
 // for c16 fields; c8 fields with an odd row length -- the y pass over Nz/2+1 columns -- keep the register-I/O kernel).
 // *done = false: not applicable, the caller falls back.  d_total: rows of the peer field (peer stores only).
+// Tensor map of the TMA line pass over lines of N = 64 R complex values: 4-D {inner (as 2 n_inner reals), j, i, outer}
+// with line element n = j + R i, boxes of one row group (64 rows of B = 128 / sizeof(complex) columns).  false: the
+// shape does not qualify (unaligned rows, out of the encoder's range, no encoder): the caller keeps the older kernels.
+template <typename T>
+static bool encode_lines_tmap(CUtensorMap *tmap, const void *src, int N, int64_t line_stride, int64_t n_inner,
+                              int64_t n_outer, int64_t ostride) {
+    typedef typename C2<T>::type C;
+    const size_t cs = sizeof(C);
+    if ((reinterpret_cast<uintptr_t>(src) & 15) || ((size_t)line_stride * cs) % 16 || ((size_t)ostride * cs) % 16) return false;
+    if (2 * n_inner >= (1ll << 31) || n_outer >= (1ll << 31) || (size_t)ostride * cs >= ((size_t)1 << 40) ||
+        (size_t)(N / 64) * line_stride * cs >= ((size_t)1 << 40)) return false;
+    nbk_encode_tiled_fn enc = get_tensor_map_encoder();
+    if (!enc) return false;
+    const int R = N / 64;
+    constexpr int B = 128 / (int)sizeof(C);                    // tile width: 128-byte rows
+    const cuuint64_t gdim[4] = {(cuuint64_t)(2 * n_inner), (cuuint64_t)R, 64, (cuuint64_t)n_outer};
+    const cuuint64_t gstr[3] = {(cuuint64_t)line_stride * cs, (cuuint64_t)R * line_stride * cs, (cuuint64_t)ostride * cs};
+    const cuuint32_t box[4] = {(cuuint32_t)(2 * B), 1, 64, 1};
+    const cuuint32_t estr[4] = {1, 1, 1, 1};
+    CUresult cr = enc(tmap, sizeof(T) == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT64, 4,
+                      const_cast<void *>(src), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                      CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    return cr == CUDA_SUCCESS;                                 // a shape the encoder refuses: older kernels
+}
+
+// TMA-pipelined line pass (k_fft_lines_tma) where it applies: N in {256, 512, 1024}, 16-byte aligned rows (always true
+// for c16 fields; c8 fields with an odd row length -- the y pass over Nz/2+1 columns -- keep the register-I/O kernel).
+// *done = false: not applicable, the caller falls back.  d_total: rows of the peer field (peer stores only).
 template <typename T>
 static int launch_lines_tma(const void *src, void *dst, void *const *peer_host, int P, int N, int64_t line_stride,
                             int64_t n_inner, int64_t n_outer, int64_t outer_stride, int64_t outer_start, int inverse,
@@ -1235,22 +1457,10 @@ static int launch_lines_tma(const void *src, void *dst, void *const *peer_host, 
     const size_t cs = sizeof(C);
     if (n_outer > 1 && outer_stride == 0) return NBK_OK;
     const int64_t ostride = n_outer > 1 ? outer_stride : (int64_t)N * line_stride;
-    if ((reinterpret_cast<uintptr_t>(src) & 15) || ((size_t)line_stride * cs) % 16 || ((size_t)ostride * cs) % 16) return NBK_OK;
-    if (2 * n_inner >= (1ll << 31) || n_outer >= (1ll << 31) || (size_t)ostride * cs >= ((size_t)1 << 40) ||
-        (size_t)(N / 64) * line_stride * cs >= ((size_t)1 << 40)) return NBK_OK;
-    nbk_encode_tiled_fn enc = get_tensor_map_encoder();
-    if (!enc) return NBK_OK;
+    CUtensorMap tmap;
+    if (!encode_lines_tmap<T>(&tmap, src, N, line_stride, n_inner, n_outer, ostride)) return NBK_OK;
     const int R = N / 64;
     constexpr int B = 128 / (int)sizeof(C);                    // tile width: 128-byte rows
-    CUtensorMap tmap;
-    const cuuint64_t gdim[4] = {(cuuint64_t)(2 * n_inner), (cuuint64_t)R, 64, (cuuint64_t)n_outer};
-    const cuuint64_t gstr[3] = {(cuuint64_t)line_stride * cs, (cuuint64_t)R * line_stride * cs, (cuuint64_t)ostride * cs};
-    const cuuint32_t box[4] = {(cuuint32_t)(2 * B), 1, 64, 1};
-    const cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult cr = enc(&tmap, sizeof(T) == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT64, 4,
-                      const_cast<void *>(src), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                      CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) return NBK_OK;                     // shape the encoder refuses: older kernels
     int dtype = sizeof(T) == 4 ? NBK_F4 : NBK_F8;
     void *tw;
     int rc = get_twiddle(N, dtype, s, &tw);
@@ -1596,6 +1806,104 @@ extern "C" int nbk_fft_z_forward(const void *real, void *cplx, int dtype, int64_
                              : launch_z<double>(real, cplx, rows, (int)Nz, true, 1.0, s);
 }
 
+// Ticket counter and per-(plane, z item) epoch flags of k_fft_zy_r2c_pipe, one set per (device, stream).  Calls on one
+// stream run one after the other, so they can share a set; calls on different streams may run at the same time and
+// each stream has its own.  Streams are told apart by cudaStreamGetId, which no later stream reuses (a handle can be
+// reused after cudaStreamDestroy while the destroyed stream's work is still running).  A set stays allocated for the
+// life of the process, as the twiddle tables do: 4 bytes plus 4 per (plane, z item) of the largest call on the stream.
+struct ZyPipeSync {
+    unsigned *ticket = nullptr, *flags = nullptr;
+    int64_t n_flags = 0;
+    unsigned epoch = 0;
+};
+static std::mutex g_zy_mutex;
+static std::map<std::pair<int, unsigned long long>, ZyPipeSync> g_zy;
+
+// the pipelined z + y pass where both passes would run their TMA kernels: f8, Nz = 2M with M in {128, 256, 512},
+// Ny = 64 R with R in {4, 8, 16}, and more than D planes.  *done = false: not applicable, the caller runs the two passes.
+template <typename T>
+static int launch_zy_pipe(const void *real, void *cplx, int64_t x_n, int Ny, int Nz, cudaStream_t s, bool *done) {
+    typedef typename C2<T>::type C;
+    *done = false;
+    const int M = Nz / 2, R = Ny / 64;
+    if ((M != 128 && M != 256 && M != 512) || (R != 4 && R != 8 && R != 16) || x_n >= (1 << 20)) return NBK_OK;
+    if ((reinterpret_cast<uintptr_t>(real) & 15) || ((size_t)Nz * sizeof(T)) % 16) return NBK_OK;
+    const int64_t Nzc = M + 1;
+    CUtensorMap tmap;
+    if (!encode_lines_tmap<T>(&tmap, cplx, Ny, Nzc, Nzc, x_n, Ny * Nzc)) return NBK_OK;
+    const int dtype = sizeof(T) == 4 ? NBK_F4 : NBK_F8;
+    void *twz, *twy;
+    int rc = get_twiddle(Nz, dtype, s, &twz);
+    if (rc) return rc;
+    rc = get_twiddle(Ny, dtype, s, &twy);
+    if (rc) return rc;
+    int dev = 0, sms = 0, l2 = 0;
+    NBK_CUDA(cudaGetDevice(&dev));
+    NBK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    NBK_CUDA(cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, dev));
+    // pipeline depth: the y tiles trail the z items by D planes; the D planes waiting for their y tiles and the one
+    // being transformed take at most about half the L2
+    const int64_t plane_bytes = (int64_t)Ny * Nzc * (int64_t)sizeof(C);
+    int64_t D = (int64_t)l2 / (2 * plane_bytes) - 1;
+    if (D < 1) D = 1;
+    // a slab of at most D planes fits in half the L2 as a whole: the y pass of the two launches already reads the z
+    // rows from L2, and the single persistent kernel only adds its start-up (measured slower on 1- and 2-plane slabs)
+    if (x_n <= D) return NBK_OK;
+    // shared memory: the larger of the z row buffers and the y ring, the twiddle tables, the mbarriers, the ticket
+    constexpr int NW = ZY_NT / 32, B = 128 / (int)sizeof(C);
+    const int nbuf = ZY_ZBUF / M, NS = R;
+    const size_t zbytes = (size_t)NW * ZY_ZBUF * sizeof(C), ybytes = (size_t)NS * 64 * B * sizeof(C);
+    const size_t smem = (zbytes > ybytes ? zbytes : ybytes) + ((size_t)(2 * M + 7 * (M / 8) + 56) + Ny + 64) * sizeof(C) +
+                        (size_t)(NW * nbuf + NS) * 8 + 16;
+    NBK_CHECK_ARG(smem <= (size_t)227 * 1024, "fft_zy_forward: the pipelined pass does not fit in shared memory "
+                  "(Ny = %d, Nz = %d)", Ny, Nz);
+    const int nzi = Ny / (NW * ZY_ZPW), nyi = (int)((Nzc + B - 1) / B);
+    const int64_t n_items = (int64_t)(nzi + nyi) * (x_n + D);
+    unsigned *ticket, *flags, epoch;
+    {
+        unsigned long long sid = 0;
+        NBK_CUDA(cudaStreamGetId(s, &sid));
+        std::lock_guard<std::mutex> lock(g_zy_mutex);
+        ZyPipeSync &st = g_zy[std::make_pair(dev, sid)];
+        if (!st.ticket) {
+            NBK_CUDA(cudaMalloc(&st.ticket, sizeof(unsigned)));
+            NBK_CUDA(cudaMemsetAsync(st.ticket, 0, sizeof(unsigned), s));
+        }
+        if (st.n_flags < x_n * nzi) {
+            if (st.flags) NBK_CUDA(cudaFree(st.flags));
+            st.flags = nullptr;
+            st.n_flags = 0;
+            NBK_CUDA(cudaMalloc(&st.flags, (size_t)x_n * nzi * sizeof(unsigned)));
+            NBK_CUDA(cudaMemsetAsync(st.flags, 0, (size_t)x_n * nzi * sizeof(unsigned), s));
+            st.n_flags = x_n * nzi;
+        }
+        ticket = st.ticket;
+        flags = st.flags;
+        epoch = ++st.epoch;
+    }
+#define LAUNCH_ZY(LMM, RR)                                                                                           \
+    do {                                                                                                             \
+        auto kern = k_fft_zy_r2c_pipe<T, LMM, RR>;                                                                   \
+        NBK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));                \
+        int occ = 0;                                                                                                 \
+        NBK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, ZY_NT, smem));                            \
+        NBK_CHECK_ARG(occ >= 1, "fft_zy_forward: the pipelined pass cannot be resident (Ny = %d, Nz = %d)", Ny, Nz); \
+        int64_t g = (int64_t)occ * sms;                                                                              \
+        if (g > n_items) g = n_items;                                                                                \
+        kern<<<(int)g, ZY_NT, smem, s>>>(tmap, (const T *)real, (C *)cplx, (const C *)twz, (const C *)twy, (int)x_n,  \
+                                         (int)D, ticket, flags, epoch, (T)1, (T)1);                                  \
+    } while (0)
+#define LAUNCH_ZY_R(LMM) do { if (R == 16) LAUNCH_ZY(LMM, 16); else if (R == 8) LAUNCH_ZY(LMM, 8); else LAUNCH_ZY(LMM, 4); } while (0)
+    if (M == 512) LAUNCH_ZY_R(9); else if (M == 256) LAUNCH_ZY_R(8); else LAUNCH_ZY_R(7);
+#undef LAUNCH_ZY_R
+#undef LAUNCH_ZY
+    NBK_LAUNCHED();
+    *done = true;
+    return NBK_OK;
+}
+
+// z and y passes of the forward transform of x_n planes: the pipelined kernel where it applies, else the z pass and
+// then the y lines
 extern "C" int nbk_fft_zy_forward(const void *real, void *cplx, int dtype, int64_t x_n, int64_t Ny, int64_t Nz,
                                   void *stream) {
     int rc = check_dims("fft_zy_forward", dtype, 1, Ny, Nz);
@@ -1603,6 +1911,11 @@ extern "C" int nbk_fft_zy_forward(const void *real, void *cplx, int dtype, int64
     if (x_n <= 0) return NBK_OK;
     cudaStream_t s = (cudaStream_t)stream;
     int64_t Nzc = Nz / 2 + 1;
+    if (dtype == NBK_F8) {
+        bool done = false;
+        rc = launch_zy_pipe<double>(real, cplx, x_n, (int)Ny, (int)Nz, s, &done);
+        if (rc || done) return rc;
+    }
     rc = (dtype == NBK_F4) ? launch_z<float>(real, cplx, x_n * Ny, (int)Nz, true, 1.0, s)
                            : launch_z<double>(real, cplx, x_n * Ny, (int)Nz, true, 1.0, s);
     if (rc) return rc;

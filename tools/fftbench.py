@@ -5,8 +5,9 @@
 
 Every case is timed with CUDA events after warm-up (median of --reps calls).  Effective bandwidth counts 6x the real
 field's bytes per transform (three passes, each one read and one write of a field of about that size) and is compared
-with the 3.35 TB/s HBM3 data-sheet figure of the H100 SXM.  For sides that are not powers of two the three passes of
-the r2c (z, y, x) are also timed one by one: the mixed-radix passes, and the Bluestein ones on axes whose side has a
+with the 3.35 TB/s HBM3 data-sheet figure of the H100 SXM.  The three passes of the r2c (z, y, x) are also timed one by
+one: for power-of-two sides the z pass, the y lines, the x lines and "zy", the z and y passes as the r2c runs them (one
+pipelined kernel where it applies); otherwise the mixed-radix passes, and the Bluestein ones on axes whose side has a
 prime factor above 7.  The card's name and power limit are printed with the numbers.
 """
 import argparse
@@ -61,6 +62,14 @@ def _passes(pm, r, c, warmup, reps):
     Nzc = Nz // 2 + 1
     rp, cp = ctypes.c_void_p(r.value.data_ptr()), ctypes.c_void_p(c.value.data_ptr())
     out = {}
+    if pm.pow2:
+        # the z pass, the y lines and the x lines one by one, and "zy": the z and y passes as the r2c runs them
+        # (nbk_fft_zy_forward: one pipelined kernel where it applies)
+        out["z"] = _time(lambda: _lib.check(L.nbk_fft_z_forward(rp, cp, code, Nx * Ny, Nz, None)), warmup, reps)
+        out["y"] = _time(lambda: _lib.check(L.nbk_fft_lines(cp, code, Ny, Nzc, Nzc, Nx, Ny * Nzc, 0, 1.0, None)), warmup, reps)
+        out["x"] = _time(lambda: _lib.check(L.nbk_fft_lines(cp, code, Nx, Ny * Nzc, Ny * Nzc, 1, 0, 0, 1.0, None)), warmup, reps)
+        out["zy"] = _time(lambda: _lib.check(L.nbk_fft_zy_forward(rp, cp, code, Nx, Ny, Nz, None)), warmup, reps)
+        return {k: round(v, 3) for k, v in out.items()}
     zp, yp, xp = pm._z_pass(), pm._line_pass(1), pm._line_pass(0)
     out["z"] = _time(lambda: _lib.check(zp(rp, cp, code, Nx * Ny, Nz, 0, 1.0, None)), warmup, reps)
     out["y"] = _time(lambda: _lib.check(yp(cp, cp, code, Ny, Nzc, Nzc, Nx, Ny * Nzc, 0, 1.0, None)), warmup, reps)
@@ -84,8 +93,7 @@ def run_case(spec, warmup, reps, card):
     res["r2c_ns_per_cell"] = round(ms * 1e6 / n ** 3, 4)
     res["r2c_GBps"] = round(6 * field_bytes / (ms * 1e-3) / 1e9, 1)
     res["r2c_frac_hbm_peak"] = round(6 * field_bytes / (ms * 1e-3) / HBM_PEAK, 3)
-    if not pm.pow2:
-        res["r2c_passes_ms"] = _passes(pm, r, c, warmup, reps)
+    res["r2c_passes_ms"] = _passes(pm, r, c, warmup, reps)
     if with_c2r:
         ms = _time(lambda: c.c2r(out=r), warmup, reps)
         res["c2r_ms"] = round(ms, 3)
