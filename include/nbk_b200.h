@@ -423,6 +423,23 @@ int nbk_threeptcf(const double *ppos, const double *pw, const int64_t *chunk_fir
                   int nedges, const int *poles_host, int npoles, const double *coef_host, double *work, double *zeta,
                   uint64_t *npairs, uint64_t *candidates, void *stream);
 
+/* FFT bispectrum of a periodic box (algorithms/bispectrum.py: FFTBispectrum; DESIGN.md 4.14).  At most
+ * nbk_bispec_max_shells() k shells.
+ *   fill       : one pass over the Hermitian-compressed Fourier slab cplx (layout / start / count as nbk_power_bin takes
+ *                them; NBK_LAYOUT_FULLZ is refused) writes shells [shell0, shell0 + nshell) of the nedges - 1 shells of
+ *                k2edges_host (squared k edges): out[s][slab] = c * 1_S (complex of dtype) or, indicator != 0, the
+ *                complex f8 indicator 1_S, s = 0 .. nshell - 1, out_stride complex elements apart.  A mode is in shell
+ *                b - 1 when nbk_power_bin puts it in bin b at float32 coordinates; the k = 0 mode is in no shell.
+ *   triple_sum : fields holds nfield real fields of ncell values (dtype), field_stride elements apart; triples ntri
+ *                device int triples (i, j, l) of slots < nfield.  Accumulates (device, zero first)
+ *                out[t] += sum_x f_i f_j f_l, products and sums in float64. */
+int nbk_bispec_max_shells(void);
+int nbk_bispec_fill(const void *cplx, int dtype, const int64_t *nmesh_host, const double *box_host, int layout, int64_t start,
+                    int64_t count, const double *k2edges_host, int nedges, int shell0, int nshell, int indicator, void *out,
+                    int64_t out_stride, void *stream);
+int nbk_bispec_triple_sum(const void *fields, int dtype, int64_t field_stride, int nfield, int64_t ncell, const int *triples,
+                          int64_t ntri, double *out, void *stream);
+
 /* Cylindrical groups (algorithms/cgm.py: CylindricalGroups; DESIGN.md 4.9).  Rows key-sorted on a grid of ncell_host[d]
  * cells of side box[d] / ncell[d] as for nbk_paircount: spos double [n][3] (periodic: already wrapped), sprio[n] the
  * distinct global priority of each sorted row, perm[n] its row before sorting; rows with perm < n_own are owned, the

@@ -29,6 +29,7 @@ SOURCES = [
     ("fibercollisions.cu", ["--fmad=false"]),
     ("zhist.cu", ["--fmad=false"]),
     ("hod.cu", ["--fmad=false"]),
+    ("bispectrum.cu", ["--fmad=false"]),
 ]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ARCH + [ "-O3", "-lineinfo", "-std=c++17",
@@ -45,7 +46,7 @@ def _nvcc():
 def _stamp(path, flags):
     h = hashlib.sha1()
     for dep in [path, os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "pc_cells.cuh"),
-                os.path.join(CSRC, "splev.cuh"),
+                os.path.join(CSRC, "splev.cuh"), os.path.join(CSRC, "kshell.cuh"),
                 os.path.join(CSRC, "ylm_table.inc"),
                 os.path.join(HERE, "..", "include", "nbk_b200.h")]:
         with open(dep, "rb") as f:

@@ -1,4 +1,5 @@
 from .fftpower import FFTPower, FFTBase, ProjectedFFTPower, project_to_basis
+from .bispectrum import FFTBispectrum
 from .fftcorr import FFTCorr
 from .fftrecon import FFTRecon
 from .fof import FOF
@@ -14,5 +15,5 @@ from .convpower import ConvolvedFFTPower, FKPCatalog, FKPWeightFromNbar, FKPCata
 FKPPower = ConvolvedFFTPower
 
 __all__ = ['FOF', 'CylindricalGroups', 'KDDensity', 'FiberCollisions', 'RedshiftHistogram', 'SimulationBoxPairCount', 'SimulationBox2PCF', 'SimulationBox3PCF', 'SurveyDataPairCount',
-           'SurveyData2PCF', 'SurveyData3PCF', 'FFTCorr', 'FFTRecon', 'FFTPower', 'ProjectedFFTPower', 'FFTBase', 'project_to_basis', 'ConvolvedFFTPower', 'FKPPower', 'FKPCatalog',
+           'SurveyData2PCF', 'SurveyData3PCF', 'FFTCorr', 'FFTRecon', 'FFTPower', 'FFTBispectrum', 'ProjectedFFTPower', 'FFTBase', 'project_to_basis', 'ConvolvedFFTPower', 'FKPPower', 'FKPCatalog',
            'FKPWeightFromNbar', 'FKPCatalogMesh']

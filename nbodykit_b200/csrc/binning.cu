@@ -8,6 +8,7 @@
 // (k_d = fl32(f32(j_d)*f32(2 pi/L_d)), k^2 = fl32(fl32(kx^2+ky^2)+kz^2), |k| = sqrt_rn, mu = div_rn)
 // is part of the bit-exact contract (SURVEY B.5; pinned by nbodykit/tests/data/dataset_2d.json).
 #include "common.cuh"
+#include "kshell.cuh"
 #include <algorithm>
 #include <map>
 #include <mutex>
@@ -17,45 +18,6 @@
 #include <stdlib.h>
 
 #define NBK_MAX_ELL 8
-
-// ---------------------------------------------------------------------------------------------
-// index helpers: element e of a slab -> integer frequency labels (jx, jy, jz)
-// ---------------------------------------------------------------------------------------------
-struct SlabGeom {
-    int N[3];        // Nx, Ny, Nz of the full mesh
-    int Nzc;         // stored length of the last axis
-    int transposed;  // 0: [x_n][Ny][Nzc]   1: [y_n][Nx][Nzc]
-    int start, count;  // owned range along the first stored axis
-    int D1;          // length of the second stored axis
-};
-
-static int make_slab(const int64_t *nmesh, int transposed, int64_t start, int64_t count, int hermitian, SlabGeom &g) {
-    for (int d = 0; d < 3; d++) {
-        NBK_CHECK_ARG(nmesh[d] > 0 && nmesh[d] < (1 << 24), "bad Nmesh[%d]=%lld", d, (long long)nmesh[d]);
-        g.N[d] = (int)nmesh[d];
-    }
-    // `transposed` carries the layout bits: NBK_LAYOUT_TRANSPOSED (first stored axis is y) and NBK_LAYOUT_FULLZ (the
-    // last axis holds all Nz modes: complex-dtype meshes, real-space statistics)
-    const bool fullz = (transposed & NBK_LAYOUT_FULLZ) != 0;
-    transposed &= NBK_LAYOUT_TRANSPOSED;
-    g.Nzc = (hermitian && !fullz) ? g.N[2] / 2 + 1 : g.N[2];
-    g.transposed = transposed ? 1 : 0;
-    int D0 = transposed ? g.N[1] : g.N[0];
-    g.D1 = transposed ? g.N[0] : g.N[1];
-    NBK_CHECK_ARG(start >= 0 && count >= 0 && start + count <= D0, "bad slab range [%lld,+%lld) of %d",
-                  (long long)start, (long long)count, D0);
-    g.start = (int)start;
-    g.count = (int)count;
-    return NBK_OK;
-}
-
-__device__ __forceinline__ void slab_freqs(const SlabGeom &g, int i0, int i1, int kz, int &jx, int &jy, int &jz) {
-    int a = nbk_freq(g.start + i0, g.transposed ? g.N[1] : g.N[0]);
-    int b = nbk_freq(i1, g.transposed ? g.N[0] : g.N[1]);
-    jx = g.transposed ? b : a;
-    jy = g.transposed ? a : b;
-    jz = nbk_freq(kz, g.N[2]);
-}
 
 // ---------------------------------------------------------------------------------------------
 // compensation: v /= prod_d f(w_d), w_d = 2 pi j_d / N_d.  The factor is separable, so three 1-D
@@ -317,16 +279,6 @@ struct BinParams {
     double volume;
 };
 
-// number of edges <= x  (numpy.digitize, right=False, increasing edges)
-__device__ __forceinline__ int digitize(const double *__restrict__ edges, int n, double x) {
-    int lo = 0, hi = n;
-    while (lo < hi) {
-        int mid = (lo + hi) >> 1;
-        if (edges[mid] <= x) lo = mid + 1; else hi = mid;
-    }
-    return lo;
-}
-
 __device__ __forceinline__ double legendre(int ell, double x) {
     if (ell == 0) return 1.0;
     double p0 = 1.0, p1 = x;
@@ -484,15 +436,7 @@ k_power_bin(const T *__restrict__ c1, const T *__restrict__ c2, BinParams P, con
                     }
                 }
                 // numpy.digitize(k2, edges2): number of edges <= k2
-                int b;
-                if (uniform) {
-                    double t = (knorm - kmin) * inv_dk;
-                    b = t < 0.0 ? 0 : (t >= (double)nedge ? nedge : (int)t + 1);
-                    while (b > 0 && k2d < s_k2[b - 1]) b--;
-                    while (b < nedge && k2d >= s_k2[b]) b++;
-                } else {
-                    b = digitize(s_k2, nedge, k2d);
-                }
+                int b = nbk_k2_bin(s_k2, nedge, k2d, knorm, kmin, inv_dk, uniform);
                 int dm = 0;
                 for (int i = 0; i <= P.Nmu; i++) dm += (s_mu[i] <= mu) ? 1 : 0;
                 key = b * (P.Nmu + 2) + dm;
@@ -786,16 +730,8 @@ static int power_bin_impl(const void *c1, const void *c2, const void *c3, int dt
         ctz = t[2];
     }
     // are the k edges uniformly spaced (numpy.arange)?  then bins start from a closed-form guess
-    double kmin = 0.0, inv_dk = 0.0;
-    int uniform = 0;
-    if (Nx >= 1 && k2edges[0] >= 0.0) {
-        kmin = sqrt(k2edges[0]);
-        double dk = (sqrt(k2edges[Nx]) - kmin) / Nx;
-        uniform = dk > 0.0;
-        for (int i = 0; i <= Nx && uniform; i++)
-            if (fabs(sqrt(k2edges[i]) - (kmin + i * dk)) > 1e-3 * dk) uniform = 0;
-        if (uniform) inv_dk = 1.0 / dk;
-    }
+    double kmin, inv_dk;
+    const int uniform = nbk_k2_uniform(k2edges, Nx, &kmin, &inv_dk);
     if (dtype == NBK_F4) return launch_bin_ell<float>(c1, c2, P, d_k2, d_mu, nsum, xsum, musum, ysum, kmin, inv_dk, uniform, ct0, ct1, ctz, s);
     return launch_bin_ell<double>(c1, c2, P, d_k2, d_mu, nsum, xsum, musum, ysum, kmin, inv_dk, uniform, ct0, ct1, ctz, s);
 }
