@@ -233,6 +233,19 @@ int nbk_power_bin(const void *c1, const void *c2, int dtype, int is_p3d, double 
                   const double *los_host, const int *ells_host, int Nell, int hermitian, int comp1,
                   int comp2, int real_input, const double *coord_unit_host, int64_t *nsum, double *xsum, double *musum, double *ysum, void *stream);
 
+/* The last pass of nbk_r2c fused with the FFTPower mode '1d' auto power of nbk_power_bin, for one rank: cplx holds the
+ * whole Hermitian-compressed mesh after nbk_fft_zy_forward.  Runs the x pass scaled by extra_scale / (Nx*Ny*Nz) and
+ * bins each mode as nbk_power_bin(c1 = cplx, c2 = NULL, is_p3d = 0, clear_zero = 1, coord_dtype = 4, ells = {0},
+ * hermitian = 1, comp1 = comp2 = comp, musum = NULL) would bin the transformed field, without storing it: cplx is left
+ * as it was.  Outputs as nbk_power_bin's (nb = (Nx+2)*3, accumulated into; the imaginary parts are not touched).
+ * *fused = 0: the case does not take the fused kernel (f4 fields, line of sight not along z, mu edges other than
+ * {-1, 1}, Nx not in {256, 512, 1024}, too many k bins for shared memory); nothing ran, and the caller runs the x pass with nbk_fft_lines
+ * and then nbk_power_bin. */
+int nbk_fft_x_power_bin(void *cplx, int dtype, const int64_t *nmesh_host, const double *boxsize_host,
+                        double extra_scale, double volume, const double *k2edges_host, int Nx,
+                        const double *muedges_host, int Nmu, const double *los_host, int comp, int64_t *nsum,
+                        double *xsum, double *ysum, int *fused, void *stream);
+
 /* nbk_power_bin with a third field: c2_mirror stands for c2 at the UNSTORED mirror mode -k of every mode with
  * 0 < j_z < N_z/2, i.e. the mirror's share of the sum is conj(c1 conj(c2_mirror)) V instead of the (anti-)Hermitian
  * fold of c1 conj(c2).  This is what a full complex ('c16') mesh gives the reference when c2 carries a factor that is

@@ -65,6 +65,7 @@ SIGNATURES = {
                        _i, _i, _i, _i, _i, _pd, _vp, _vp, _vp, _vp, _vp], _i),
     "nbk_power_bin2": ([_vp, _vp, _vp, _i, _i, _d, _i, _pi64, _pd, _i, _i64, _i64, _i, _pd, _i, _pd, _i, _pd, _pi,
                         _i, _i, _i, _i, _i, _pd, _vp, _vp, _vp, _vp, _vp], _i),
+    "nbk_fft_x_power_bin": ([_vp, _i, _pi64, _pd, _d, _d, _pd, _i, _pd, _i, _pd, _i, _vp, _vp, _vp, _pi, _vp], _i),
     "nbk_ylm_mul_complex_acc2": ([_vp, _vp, _vp, _i, _i, _i, _pi64, _pd, _i, _i64, _i64, _vp], _i),
     "nbk_hermitian_expand": ([_vp, _vp, _i, _pi64, _vp], _i),
     "nbk_hermitian_compress": ([_vp, _vp, _i, _i64, _i64, _vp], _i),

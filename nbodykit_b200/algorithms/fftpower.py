@@ -12,6 +12,7 @@ as the reference (fftpower.py:146-359).  What differs is where the O(Nmesh^3) wo
   x-slab + 4 MPI allreduce      :507-701      arithmetic bit-identical to the reference's digitize, f64
                                               accumulators, one NCCL all-reduce of the packed histogram
 """
+import ctypes
 import logging
 
 import numpy
@@ -71,9 +72,11 @@ class FFTBase(object):
         self.comm = comm
         return self
 
-    def _compute_3d_power(self, first, second):
+    def _compute_3d_power(self, first, second, x_pending=False):
         """the two complex fields whose product is the 3-D power, plus attrs (fftpower.py:91-143).
-        The product c1*conj(c2)*V with the zero mode cleared is formed inside the binning kernel."""
+        The product c1*conj(c2)*V with the zero mode cleared is formed inside the binning kernel.
+        x_pending (auto power only): the field may come without its x pass, which project_to_basis_device then runs
+        fused with the binning (CatalogMesh.to_complex_field)."""
         attrs = {}
         attrs.update(self.attrs)
 
@@ -81,6 +84,8 @@ class FFTBase(object):
             # a CatalogMesh whose only action is its window compensation hands over the uncompensated field
             # and the name of the transfer function; the binning kernel applies it on the fly
             if hasattr(src, 'compute_complex_deferred'):
+                if x_pending and first is second:
+                    return src.compute_complex_deferred(Nmesh=self.attrs['Nmesh'], x_pending=True)
                 return src.compute_complex_deferred(Nmesh=self.attrs['Nmesh'])
             return src.compute(mode='complex', Nmesh=self.attrs['Nmesh']), None
         c1, comp1 = field_of(first)
@@ -134,8 +139,11 @@ class FFTPower(FFTBase):
     def run(self):
         if self.attrs['mode'] == "1d":
             self.attrs['Nmu'] = 1
+        # the 1d auto power on one rank takes the x pass fused with the binning (the partial field stays in here)
+        x_pending = (self.attrs['mode'] == "1d" and self.first is self.second and not self.attrs['poles']
+                     and self.comm.size == 1)
         with stage("H:compute_fields"):
-            c1, c2, attrs = self._compute_3d_power(self.first, self.second)
+            c1, c2, attrs = self._compute_3d_power(self.first, self.second, x_pending=x_pending)
         dk = self.attrs['dk']
         kmin = self.attrs['kmin']
         kmax = self.attrs['kmax']
@@ -359,23 +367,49 @@ def project_to_basis_device(y3d, edges, los=[0, 0, 1], poles=[], coord_dtype="f4
     herm = 0 if (is_real or not y3d.compressed) else (2 if antihermitian else 1)
     if mirror is not None and (herm != 1 or second is None or tuple(mirror.value.shape) != tuple(y3d.value.shape)):
         raise ValueError("a mirror field needs a Hermitian-compressed pair of fields of the same shape")
-    with stage("power_bin"):
-        fn = lib().nbk_power_bin if mirror is None else lib().nbk_power_bin2
-        extra = () if mirror is None else (_ptr(mirror.value),)
-        row, keep = 0, []
-        for i, grp in enumerate(groups):
-            first = i == 0
-            check(fn(
-                _ptr(y3d.value), _ptr(second.value) if second is not None else None, *extra, _CODE[pm.typestr],
-                1 if is_p3d else 0, float(volume), 1 if clear_zero else 0, pm._nmesh_c, pm._box_c, tr, start, count,
-                _los_coord_mode(los, coord_dtype), _lib.darr(x2edges), Nx, _lib.darr(muedges), Nmu, _lib.darr(los_f),
-                _lib.i32arr(grp), len(grp), herm, _lib.COMP.get(compensation[0], 0),
-                _lib.COMP.get(compensation[1], 0), 1 if is_real else 0, coord_unit,
-                _ptr(nsum if first else spare_n), _ptr(xsum if first else spare_x),
-                _ptr(musum) if (need_mu and first) else None, _ptr(facc[(2 + 2 * row) * nb:]), _stream()),
-                "nbk_power_bin")
-            keep += range(row if first else row + 1, row + len(grp))
-            row += len(grp)
+    row, keep = 0, []
+    # a field handed over before its x pass (FFTPower mode '1d', CatalogMesh.to_complex_field): the x pass runs fused
+    # with the binning where nbk_fft_x_power_bin takes the case, else it completes the field before the usual binning
+    x_scale = getattr(y3d, '_x_scale', None)
+    fused = False
+    if x_scale is not None:
+        if (not is_p3d and second is None and mirror is None and Nell == 1 and herm == 1 and not need_mu
+                and clear_zero and comm.size == 1 and compensation[0] == compensation[1]
+                and _los_coord_mode(los, coord_dtype) == 4):
+            flag = ctypes.c_int(0)
+            with stage("fft_x_bin"):
+                check(lib().nbk_fft_x_power_bin(
+                    _ptr(y3d.value), _CODE[pm.typestr], pm._nmesh_c, pm._box_c, float(x_scale), float(volume),
+                    _lib.darr(x2edges), Nx, _lib.darr(muedges), Nmu, _lib.darr(los_f),
+                    _lib.COMP.get(compensation[0], 0), _ptr(nsum), _ptr(xsum), _ptr(facc[2 * nb:]),
+                    ctypes.byref(flag), _stream()), "nbk_fft_x_power_bin")
+            fused = flag.value == 1
+            keep = [0]
+        if not fused:
+            Nx_, Ny_, Nz_ = [int(v) for v in pm.Nmesh]
+            with stage("fft_x"):
+                check(lib().nbk_fft_lines(_ptr(y3d.value), _CODE[pm.typestr], Nx_, Ny_ * (Nz_ // 2 + 1),
+                                          Ny_ * (Nz_ // 2 + 1), 1, 0, 0, float(x_scale) / (Nx_ * Ny_ * Nz_), _stream()),
+                      "nbk_fft_lines")
+            y3d._x_scale = None
+    if not fused:
+        with stage("power_bin"):
+            fn = lib().nbk_power_bin if mirror is None else lib().nbk_power_bin2
+            extra = () if mirror is None else (_ptr(mirror.value),)
+            row, keep = 0, []
+            for i, grp in enumerate(groups):
+                first = i == 0
+                check(fn(
+                    _ptr(y3d.value), _ptr(second.value) if second is not None else None, *extra, _CODE[pm.typestr],
+                    1 if is_p3d else 0, float(volume), 1 if clear_zero else 0, pm._nmesh_c, pm._box_c, tr, start, count,
+                    _los_coord_mode(los, coord_dtype), _lib.darr(x2edges), Nx, _lib.darr(muedges), Nmu, _lib.darr(los_f),
+                    _lib.i32arr(grp), len(grp), herm, _lib.COMP.get(compensation[0], 0),
+                    _lib.COMP.get(compensation[1], 0), 1 if is_real else 0, coord_unit,
+                    _ptr(nsum if first else spare_n), _ptr(xsum if first else spare_x),
+                    _ptr(musum) if (need_mu and first) else None, _ptr(facc[(2 + 2 * row) * nb:]), _stream()),
+                    "nbk_power_bin")
+                keep += range(row if first else row + 1, row + len(grp))
+                row += len(grp)
     with stage("H:bin_reduce"):
         if comm.size > 1:
             comm.allreduce_tensor(nsum)

@@ -747,6 +747,59 @@ extern "C" int nbk_power_bin(const void *c1, const void *c2, int dtype, int is_p
                           xsum, musum, ysum, stream);
 }
 
+// FFTPower mode '1d' auto power of a single-rank Hermitian-compressed field that still lacks its x pass: the x pass
+// (scaled by extra_scale / prod(N)) fused with nbk_power_bin's binning, float32 coordinates (coord_dtype 4), poles [0],
+// zero mode cleared.  *fused = 0 when the shape or the binning does not take the fused kernel (f4, line of sight not
+// along z, mu edges other than {-1, 1}, Nx not in {256, 512, 1024}, too many k bins for shared memory): nothing ran and the
+// caller finishes the transform and bins as usual.
+extern "C" int nbk_fft_x_power_bin(void *cplx, int dtype, const int64_t *nmesh, const double *box, double extra_scale,
+                                   double volume, const double *k2edges, int Nx, const double *muedges, int Nmu,
+                                   const double *los, int comp, int64_t *nsum, double *xsum, double *ysum, int *fused,
+                                   void *stream) {
+    NBK_CHECK_ARG(fused != nullptr, "fft_x_power_bin: null result flag");
+    *fused = 0;
+    NBK_CHECK_ARG(dtype == NBK_F4 || dtype == NBK_F8, "fft_x_power_bin: bad dtype %d", dtype);
+    NBK_CHECK_ARG(Nx >= 0 && Nmu >= 1, "fft_x_power_bin: need Nx >= 0 and Nmu >= 1");
+    NBK_CHECK_ARG(comp >= 0 && comp <= NBK_COMP_PCS_SHOTNOISE, "fft_x_power_bin: unknown compensation kind %d", comp);
+    SlabGeom g;
+    int rc = make_slab(nmesh, 0, 0, nmesh[0], 1, g);
+    if (rc) return rc;
+    if (Nmu != 1 || muedges[0] != -1.0 || muedges[1] != 1.0 || los[0] != 0.0 || los[1] != 0.0) return NBK_OK;
+    XBinArgs a;
+    const double TWO_PI = 6.283185307179586476925286766559;
+    for (int d = 0; d < 3; d++) {
+        NBK_CHECK_ARG(box[d] > 0, "fft_x_power_bin: bad BoxSize");
+        a.N[d] = g.N[d];
+        a.kf32[d] = (float)(TWO_PI / box[d]);
+    }
+    a.Nzc = g.Nzc;
+    a.losz32 = (float)los[2];
+    a.volume = volume;
+    a.nedge = Nx + 1;
+    cudaStream_t s = (cudaStream_t)stream;
+    double *d_k2;
+    if ((rc = get_edges(k2edges, Nx + 1, s, &d_k2))) return rc;
+    a.k2edges = d_k2;
+    a.uniform = nbk_k2_uniform(k2edges, Nx, &a.kmin, &a.inv_dk);
+    a.ct0 = a.ct1 = a.ctz = nullptr;
+    if (comp != NBK_COMP_NONE) {
+        double *t[3];
+        for (int d = 0; d < 3; d++)
+            if ((rc = get_comp_pair_table(comp, comp, g.N[d], s, &t[d]))) return rc;
+        a.ct0 = t[0];
+        a.ct1 = t[1];
+        a.ctz = t[2];
+    }
+    a.nsum = (unsigned long long *)nsum;
+    a.xsum = xsum;
+    a.ysum = ysum;
+    const double scale = extra_scale / ((double)g.N[0] * (double)g.N[1] * (double)g.N[2]);   // as nbk_r2c
+    bool done = false;
+    if ((rc = fft_x_bin_launch(cplx, dtype, scale, a, s, &done))) return rc;
+    *fused = done ? 1 : 0;
+    return NBK_OK;
+}
+
 extern "C" int nbk_power_bin2(const void *c1, const void *c2, const void *c2_mirror, int dtype, int is_p3d, double volume,
                               int clear_zero, const int64_t *nmesh, const double *box, int transposed, int64_t start,
                               int64_t count, int coord_dtype, const double *k2edges, int Nx, const double *muedges, int Nmu,

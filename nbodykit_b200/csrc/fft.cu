@@ -27,6 +27,7 @@
 // axes whose side has a larger prime factor through the Bluestein passes after them (k_fft_lines_bluestein,
 // k_fft_z_bluestein), which reuse the mixed-radix stages for their convolution.
 #include "common.cuh"
+#include "kshell.cuh"
 #include <cuda.h>      // CUtensorMap types only: the encoder comes from cudaGetDriverEntryPoint (no -lcuda)
 #include <map>
 #include <mutex>
@@ -650,23 +651,15 @@ template <int R, typename C> __device__ __forceinline__ void dftR(C (&a)[R]) {
 // the whole SM).  Also its launch bound: without it ptxas trades spills for an occupancy the ring rules out.
 __host__ __device__ constexpr int tma_ctas_per_sm(int R) { return R == 16 ? 1 : R == 4 ? 3 : 2; }
 
-// One tile of the TMA line pass: its R row groups are landing in the ring slots (g0 + j) % NS (g0 = groups this CTA
-// streamed before the tile, which also gives each slot's mbarrier phase).  The NT threads run the 64-point FFTs (warp
-// w owns groups w, w + NW, ...; warps beyond R wait), the radix-R combine and the stores, then free the R slots: on
-// return they may be refilled.
-template <typename T, int R, int B, int NT, bool PEER>
-__device__ __forceinline__ void lines_tma_tile(typename C2<T>::type *ring, uint64_t *bars, int NS, int g0,
-                                               const typename C2<T>::type *twN, const typename C2<T>::type *tw64,
-                                               typename C2<T>::type *dst, const PeerPtrs<typename C2<T>::type> &peers,
-                                               int64_t line_stride, int64_t n_inner, int64_t outer_stride, int n_per,
-                                               int64_t d_total, int64_t outer_start, int64_t outer, int64_t inner0,
-                                               T sgn, T scale) {
+// The 64-point FFTs of a tile's R row groups (warp-local: two radix-8 stages in place); position 8 t + m of a slot
+// then holds frequency t + 8 m.  Ends with a CTA barrier.
+template <typename T, int R, int B, int NT>
+__device__ __forceinline__ void lines_tma_groups(typename C2<T>::type *ring, uint64_t *bars, int NS, int g0,
+                                                 const typename C2<T>::type *tw64, T sgn) {
     typedef typename C2<T>::type C;
-    constexpr int S = 64, NW = NT / 32, SLOT = S * B;
+    constexpr int NW = NT / 32, SLOT = 64 * B;
     static_assert((8 * B) % 32 == 0 && (R % NW == 0 || NW % R == 0), "tile geometry");
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int bvalid = (int)((n_inner - inner0) < B ? (n_inner - inner0) : B);
-    // ---- 64-point FFT of my row group (warp-local: two radix-8 stages in place)
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     for (int gw = warp; gw < R; gw += NW) {
         const int g = g0 + gw, slot = g % NS;
         fm_mbar_wait(&bars[slot], (unsigned)((g / NS) & 1));
@@ -698,6 +691,24 @@ __device__ __forceinline__ void lines_tma_tile(typename C2<T>::type *ring, uint6
         }
     }
     __syncthreads();
+}
+
+// One tile of the TMA line pass: its R row groups are landing in the ring slots (g0 + j) % NS (g0 = groups this CTA
+// streamed before the tile, which also gives each slot's mbarrier phase).  The NT threads run the 64-point FFTs (warp
+// w owns groups w, w + NW, ...; warps beyond R wait), the radix-R combine and the stores, then free the R slots: on
+// return they may be refilled.
+template <typename T, int R, int B, int NT, bool PEER>
+__device__ __forceinline__ void lines_tma_tile(typename C2<T>::type *ring, uint64_t *bars, int NS, int g0,
+                                               const typename C2<T>::type *twN, const typename C2<T>::type *tw64,
+                                               typename C2<T>::type *dst, const PeerPtrs<typename C2<T>::type> &peers,
+                                               int64_t line_stride, int64_t n_inner, int64_t outer_stride, int n_per,
+                                               int64_t d_total, int64_t outer_start, int64_t outer, int64_t inner0,
+                                               T sgn, T scale) {
+    typedef typename C2<T>::type C;
+    constexpr int S = 64, SLOT = S * B;
+    const int tid = threadIdx.x;
+    const int bvalid = (int)((n_inner - inner0) < B ? (n_inner - inner0) : B);
+    lines_tma_groups<T, R, B, NT>(ring, bars, NS, g0, tw64, sgn);
     // ---- radix-R combine across the groups, registers -> global frequency rows k + 64 m
     {
         const int base = g0 % NS;
@@ -1495,6 +1506,256 @@ static int launch_lines_tma(const void *src, void *dst, void *const *peer_host, 
     NBK_LAUNCHED();
     *done = true;
     return NBK_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// x pass fused with the FFTPower 1d auto-power binning (one rank: lines of N = 64 R strided by Ny*Nzc).  FFTPower keeps
+// only the binned sums, so the transformed field is never stored: the pass reads the z + y output once, writes nothing.
+// A tile runs the row-group FFTs and the radix-R combine of k_fft_lines_tma and scales each mode exactly as its store
+// does.  The scaled modes go back into the tile's R slots column by column ([b][64] per slot, the position XOR-swizzled
+// by b, so that the combine's writes and the binning's reads are both free of bank conflicts).  A warp then bins 32
+// consecutive j = jx >= 0 of one (ky, kz) column together with their mirrors -j, which have the same |k| and mu for a
+// line of sight along z.  |k| grows with j, so equal bins are contiguous runs of lanes, which a segmented shuffle
+// reduction folds into one shared-memory atomic per run; each CTA adds its sums to the global ones at the end.
+// The bin of a mode must be the one nbk_power_bin gives it (binning.cu is built with --fmad=false, this file is not), so
+// its arithmetic uses explicit round-to-nearest intrinsics throughout.
+// The ring set-up and refill repeat k_fft_lines_tma's on purpose: the same code behind a shared helper struct measured
+// 0.8 ms slower at 1024^3 f8 (8.7 against 7.9 ms per call on an H100 80GB HBM3, 700 W).
+template <typename T, int R, int B, int NT>
+__global__ void __launch_bounds__(NT, tma_ctas_per_sm(R))
+k_fft_x_bin(const __grid_constant__ CUtensorMap tmap, const typename C2<T>::type *__restrict__ twg, int64_t n_inner,
+            int64_t n_tiles, T scale, int NS, const XBinArgs a) {
+    typedef typename C2<T>::type C;
+    constexpr int S = 64, N = S * R, SLOT = S * B, NW = NT / 32, IT = S * B / NT;
+    static_assert((S * B) % NT == 0 && B <= 32, "tile geometry");
+    extern __shared__ __align__(1024) unsigned char smem_raw[];
+    C *ring = reinterpret_cast<C *>(smem_raw);                 // [NS][64][B]
+    C *twN = ring + (size_t)NS * SLOT;
+    C *tw64 = twN + N;
+    uint64_t *bars = reinterpret_cast<uint64_t *>(tw64 + S);   // [NS]
+    double *s_k2 = reinterpret_cast<double *>(bars + NS);      // [nedge]
+    const int nedge = a.nedge, nkb = nedge + 1;
+    double *s_x = s_k2 + nedge;                                // per k bin (mu bin 1): sum |k| w, sum P w, sum w
+    double *s_p = s_x + nkb;
+    unsigned *s_n = reinterpret_cast<unsigned *>(s_p + nkb);
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (tid == 0) {
+        for (int i = 0; i < NS; i++) fm_mbar_init(&bars[i], 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    for (int i = tid; i < N; i += NT) twN[i] = twg[i];
+    for (int i = tid; i < S; i += NT) tw64[i] = twg[i * R];
+    for (int i = tid; i < nedge; i += NT) s_k2[i] = a.k2edges[i];
+    for (int i = tid; i < nkb; i += NT) { s_x[i] = 0.0; s_p[i] = 0.0; s_n[i] = 0u; }
+    __syncthreads();
+    const int64_t first = blockIdx.x;
+    const int my_tiles = first < n_tiles ? (int)((n_tiles - first + gridDim.x - 1) / gridDim.x) : 0;
+    const int G = my_tiles * R;
+    int issued = 0;
+    auto issue = [&](int g) {
+        const int it = g / R, j = g - it * R;
+        const int64_t inner0 = (first + (int64_t)it * gridDim.x) * B;
+        const int slot = g % NS;
+        fm_mbar_expect_tx(&bars[slot], (unsigned)(SLOT * sizeof(C)));
+        fm_tma_load_4d(ring + (size_t)slot * SLOT, &tmap, (int)(2 * inner0), j, 0, 0, &bars[slot]);
+    };
+    if (tid == 0) {
+        const int upto = G < NS ? G : NS;
+        for (; issued < upto; issued++) issue(issued);
+    }
+    const int Ny = a.N[1], Nz = a.N[2], Nzc = a.Nzc;
+    const float kfx = a.kf32[0], kfy = a.kf32[1], kfz = a.kf32[2];
+    const unsigned FULL = 0xffffffffu;
+    for (int it = 0; it < my_tiles; it++) {
+        const int inner0 = (int)((first + (int64_t)it * gridDim.x) * B);
+        const int bvalid = (int)((n_inner - inner0) < B ? (n_inner - inner0) : B);
+        const int g0 = it * R, base = g0 % NS;
+        lines_tma_groups<T, R, B, NT>(ring, bars, NS, g0, tw64, (T)1);
+        // ---- radix-R combine, scaled as the store of k_fft_lines_tma scales, back into the slots by column
+        C v[IT][R];
+#pragma unroll
+        for (int i = 0; i < IT; i++) {
+            const int w = tid + NT * i, b = w % B, k = w / B;
+            const int pos = ((k & 7) << 3) | (k >> 3);
+#pragma unroll
+            for (int j = 0; j < R; j++) {
+                int sj = base + j;
+                if (sj >= NS) sj -= NS;
+                const C x = ring[(size_t)sj * SLOT + pos * B + b];
+                v[i][j] = j ? cmul(x, twN[j * k]) : x;
+            }
+            dftR<R, C>(v[i]);
+#pragma unroll
+            for (int m = 0; m < R; m++) v[i][m] = C{v[i][m].x * scale, v[i][m].y * scale};
+        }
+        __syncthreads();
+#pragma unroll
+        for (int i = 0; i < IT; i++) {
+            const int w = tid + NT * i, b = w % B, k = w / B;
+#pragma unroll
+            for (int m = 0; m < R; m++) {
+                int sm = base + m;
+                if (sm >= NS) sm -= NS;
+                ring[(size_t)sm * SLOT + b * S + (k ^ b)] = v[i][m];
+            }
+        }
+        __syncthreads();
+        // ---- binning.  Mode K = jx mod N of column b sits in slot base + K / 64 at b * 64 + ((K % 64) ^ b).
+        // stats of mode j of column b, plus its mirror N - j when `pair`: k bin, mu bin, weight, weighted |k| and P
+        auto mode_stats = [&](int b, int j, bool pair, int &kb, int &dm, unsigned &cnt, double &xs, double &ps) {
+            const int inner = inner0 + b, iy = inner / Nzc, kz = inner - iy * Nzc;
+            const int jx = nbk_freq(j, N), jy = nbk_freq(iy, Ny), jz = nbk_freq(kz, Nz);
+            const float kx = __fmul_rn((float)jx, kfx), ky = __fmul_rn((float)jy, kfy), kzv = __fmul_rn((float)jz, kfz);
+            const float k2 = __fadd_rn(__fadd_rn(__fmul_rn(kx, kx), __fmul_rn(ky, ky)), __fmul_rn(kzv, kzv));
+            const float kn = __fsqrt_rn(k2);
+            const float mu = kn == 0.0f ? 0.0f : __fdiv_rn(__fmul_rn(kzv, a.losz32), kn);
+            kb = nbk_k2_bin(s_k2, nedge, (double)k2, (double)kn, a.kmin, a.inv_dk, a.uniform);
+            dm = (mu >= -1.0f ? 1 : 0) + (mu >= 1.0f ? 1 : 0);       // numpy.digitize(mu, [-1, 1])
+            const bool nonsing = jz > 0;                               // Hermitian weight: 1 on the kz = 0 / Nz/2 planes
+            cnt = (nonsing ? 2u : 1u) * (pair ? 2u : 1u);
+            xs = __dmul_rn((double)kn, (double)cnt);
+            int sl = base + (j >> 6);
+            if (sl >= NS) sl -= NS;
+            C c = ring[(size_t)sl * SLOT + b * S + ((j & 63) ^ b)];
+            double p = __dadd_rn(__dmul_rn((double)c.x, (double)c.x), __dmul_rn((double)c.y, (double)c.y));
+            if (pair) {
+                const int K = N - j;
+                sl = base + (K >> 6);
+                if (sl >= NS) sl -= NS;
+                c = ring[(size_t)sl * SLOT + b * S + ((K & 63) ^ b)];
+                p = __dadd_rn(p, __dadd_rn(__dmul_rn((double)c.x, (double)c.x), __dmul_rn((double)c.y, (double)c.y)));
+            }
+            double vol = a.volume;
+            if (a.ct0) vol = __dmul_rn(__dmul_rn(vol, __dmul_rn(a.ct0[j], a.ct1[iy])), a.ctz[kz]);
+            ps = (jx == 0 && jy == 0 && jz == 0) ? 0.0 : __dmul_rn(p, vol);     // the zero mode is cleared
+            if (nonsing) ps = __dmul_rn(ps, 2.0);
+        };
+        // modes outside mu bin 1 (mu == 1 on the kz axis, a rounding below -1) go straight to the global sums
+        auto add_global = [&](int key, unsigned cnt, double xs, double ps) {
+            atomicAdd(&a.nsum[key], (unsigned long long)cnt);
+            if (xs != 0.0) atomicAdd(&a.xsum[key], xs);
+            if (ps != 0.0) atomicAdd(&a.ysum[2 * key], ps);
+        };
+        for (int t = warp; t < B * R; t += NW) {
+            const int b = t / R, j = (t - b * R) * 32 + lane;      // j < N / 2: pairs (j, N - j), j = 0 alone
+            if (b >= bvalid) continue;
+            int kb, dm;
+            unsigned cnt;
+            double xs, ps;
+            mode_stats(b, j, j > 0, kb, dm, cnt, xs, ps);
+            int key = kb;
+            if (dm != 1) { add_global(kb * 3 + dm, cnt, xs, ps); key = -1; cnt = 0; xs = 0.0; ps = 0.0; }
+            // equal-key runs of lanes -> one atomic per run
+            const int prev = __shfl_up_sync(FULL, key, 1);
+            const bool head = (lane == 0) || (prev != key);
+            const unsigned heads = __ballot_sync(FULL, head);
+            if (heads == 1u) {
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) {
+                    cnt += __shfl_xor_sync(FULL, cnt, o);
+                    xs += __shfl_xor_sync(FULL, xs, o);
+                    ps += __shfl_xor_sync(FULL, ps, o);
+                }
+            } else if (heads != FULL) {
+                const int seg = __popc(heads & (FULL >> (31 - lane)));
+                const unsigned above = heads & ~((2u << lane) - 1u);
+                const int next = above ? (__ffs(above) - 1) : 32;
+                int maxrun = next - (31 - __clz(heads & ((2u << lane) - 1u)));
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) maxrun = max(maxrun, __shfl_xor_sync(FULL, maxrun, o));
+                for (int o = 1; o < maxrun; o <<= 1) {
+                    const int so = __shfl_down_sync(FULL, seg, o);
+                    const bool take = (lane + o < 32) && (so == seg);
+                    const unsigned c_o = __shfl_down_sync(FULL, cnt, o);
+                    const double x_o = __shfl_down_sync(FULL, xs, o);
+                    const double p_o = __shfl_down_sync(FULL, ps, o);
+                    if (take) { cnt += c_o; xs += x_o; ps += p_o; }
+                }
+            }
+            if (head && key >= 0) {
+                atomicAdd(&s_n[key], cnt);
+                if (xs != 0.0) atomicAdd(&s_x[key], xs);
+                if (ps != 0.0) atomicAdd(&s_p[key], ps);
+            }
+        }
+        // the Nyquist modes jx = -N/2 (no mirror), one lane per column
+        if (warp == NW - 1 && lane < bvalid) {
+            int kb, dm;
+            unsigned cnt;
+            double xs, ps;
+            mode_stats(lane, N / 2, false, kb, dm, cnt, xs, ps);
+            if (dm != 1) add_global(kb * 3 + dm, cnt, xs, ps);
+            else {
+                atomicAdd(&s_n[kb], cnt);
+                if (xs != 0.0) atomicAdd(&s_x[kb], xs);
+                if (ps != 0.0) atomicAdd(&s_p[kb], ps);
+            }
+        }
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic accesses to the slots before the next TMA writes
+        __syncthreads();
+        if (tid == 0) {
+            int upto = (it + 1) * R + NS;
+            if (upto > G) upto = G;
+            for (; issued < upto; issued++) issue(issued);
+        }
+    }
+    __syncthreads();
+    for (int i = tid; i < nkb; i += NT) {
+        const int key = i * 3 + 1;
+        if (s_n[i]) atomicAdd(&a.nsum[key], (unsigned long long)s_n[i]);
+        if (s_x[i] != 0.0) atomicAdd(&a.xsum[key], s_x[i]);
+        if (s_p[i] != 0.0) atomicAdd(&a.ysum[2 * key], s_p[i]);
+    }
+}
+
+template <typename T>
+static int launch_x_bin(void *cplx, double scale, const XBinArgs &a, cudaStream_t s, bool *done) {
+    typedef typename C2<T>::type C;
+    *done = false;
+    const int N = a.N[0];
+    if (N != 256 && N != 512 && N != 1024) return NBK_OK;
+    const int64_t line_stride = (int64_t)a.N[1] * a.Nzc;
+    CUtensorMap tmap;
+    if (!encode_lines_tmap<T>(&tmap, cplx, N, line_stride, line_stride, 1, (int64_t)N * line_stride)) return NBK_OK;
+    const int R = N / 64;
+    constexpr int B = 128 / (int)sizeof(C);
+    const size_t cs = sizeof(C), slot = (size_t)64 * B * cs;
+    // as k_fft_lines_tma's ring, less the bytes of the edges and the accumulators (one slot at N = 1024)
+    const size_t fixed = (size_t)(N + 64) * cs + 26 * 8 + (size_t)a.nedge * 8 + (size_t)(a.nedge + 1) * 20 + 64;
+    const int per_sm = tma_ctas_per_sm(R);
+    const size_t budget = (size_t)(226 * 1024) / per_sm - 1024;
+    if (budget < fixed + (size_t)(R + 1) * slot) return NBK_OK;     // too many bins for shared memory
+    int NS = (int)((budget - fixed) / slot);
+    if (NS > 26) NS = 26;
+    if (NS > 2 * R) NS = 2 * R;
+    const size_t smem = (size_t)NS * slot + fixed;
+    int dtype = sizeof(T) == 4 ? NBK_F4 : NBK_F8;
+    void *tw;
+    int rc = get_twiddle(N, dtype, s, &tw);
+    if (rc) return rc;
+    const int64_t n_tiles = (line_stride + B - 1) / B;
+    const int64_t g = n_tiles < (int64_t)NBK_SM_COUNT * per_sm ? n_tiles : (int64_t)NBK_SM_COUNT * per_sm;
+#define LAUNCH_XB(RR, NTT)                                                                                             \
+    do {                                                                                                               \
+        NBK_CUDA(cudaFuncSetAttribute(k_fft_x_bin<T, RR, B, NTT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+        k_fft_x_bin<T, RR, B, NTT><<<(int)g, NTT, smem, s>>>(tmap, (const C *)tw, line_stride, n_tiles, (T)scale, NS, a); \
+    } while (0)
+    if (R == 16) LAUNCH_XB(16, 512);
+    else if (R == 8) LAUNCH_XB(8, 256);
+    else LAUNCH_XB(4, 128);
+#undef LAUNCH_XB
+    NBK_LAUNCHED();
+    *done = true;
+    return NBK_OK;
+}
+
+// f8 only: on f4 fields the fused pass measured slower than the x pass and nbk_power_bin it replaces (the c8 x pass is
+// cheaper, the binning the same), and ptxas may contract its combine into other FMAs than k_fft_lines_tma's, which
+// moves f4 modes by an ulp
+int fft_x_bin_launch(void *cplx, int dtype, double scale, const XBinArgs &a, cudaStream_t s, bool *done) {
+    *done = false;
+    if (dtype != NBK_F8) return NBK_OK;
+    return launch_x_bin<double>(cplx, scale, a, s, done);
 }
 
 // register-I/O line pass (N >= 64; the TMA pass is tried first); peer_host != nullptr selects the peer-memory scatter

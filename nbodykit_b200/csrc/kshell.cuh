@@ -67,6 +67,24 @@ __device__ __forceinline__ int nbk_k2_bin(const double *__restrict__ k2edges, in
     return b;
 }
 
+// The last (x) pass of the forward transform fused with the FFTPower 1d auto-power binning (k_fft_x_bin in fft.cu,
+// entry point nbk_fft_x_power_bin in binning.cu).  The mode's bin is the one nbk_power_bin gives it at float32
+// coordinates with a line of sight along z and mu edges {-1, 1}; its accumulators are indexed key = kbin * 3 + mubin.
+struct XBinArgs {
+    int N[3], Nzc;
+    float kf32[3], losz32;
+    double volume;
+    const double *k2edges;     // device, nedge = Nx + 1 squared edges
+    int nedge;
+    double kmin, inv_dk;
+    int uniform;
+    const double *ct0, *ct1, *ctz;   // per-axis reciprocal window factors (both fields), null without compensation
+    unsigned long long *nsum;
+    double *xsum, *ysum;       // ysum: (re, im) pairs
+};
+// *done = false: the shape does not take the fused kernel (line length, alignment, shared memory); nothing was launched
+int fft_x_bin_launch(void *cplx, int dtype, double scale, const XBinArgs &a, cudaStream_t s, bool *done);
+
 // host side of the uniform guess: are the nedge = Nx + 1 squared edges those of numpy.arange?  Sets kmin and 1/dk.
 static inline int nbk_k2_uniform(const double *k2edges, int Nx, double *kmin, double *inv_dk) {
     *kmin = 0.0;

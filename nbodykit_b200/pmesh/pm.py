@@ -1003,6 +1003,21 @@ class RealField(Field):
             return out
         return o.cpu().numpy() if was_numpy else o
 
+    def _r2c_zy(self):
+        """the z and y passes of r2c alone, for FFTPower's x pass fused with its binning (nbk_fft_x_power_bin): a
+        ComplexField whose value is not yet a spectrum, so it must not reach anything else.  None where that path
+        does not apply: several ranks, an f4 or complex-dtype mesh, sides not powers of two, Nx outside
+        {256, 512, 1024}."""
+        pm = self.pm
+        Nx, Ny, Nz = [int(v) for v in pm.Nmesh]
+        if pm.typestr != 'f8' or pm.cplx or not pm.pow2 or pm.comm.size != 1 or Nx not in (256, 512, 1024):
+            return None
+        out = ComplexField(pm)
+        with stage("r2c_zy"):
+            check(lib().nbk_fft_zy_forward(_ptr(self.value), _ptr(out.value), _CODE[pm.typestr], Nx, Ny, Nz, _stream()),
+                  "nbk_fft_zy_forward")
+        return out
+
     def r2c(self, out=None, scale=1.0):
         """forward FFT, normalised by 1/prod(N).  out=Ellipsis has no in-place meaning here (the
         transform is out of place); the real buffer stays valid.  `scale` (extension) multiplies the

@@ -307,12 +307,18 @@ class CatalogMesh(MeshSource):
                 self.logger.info("normalized the convention to 1 + delta")
         return toret
 
-    def to_complex_field(self, out=None):
+    def to_complex_field(self, out=None, x_pending=False):
         """FFT of the 1+delta field without the intermediate normalisation / interlacing round trip:
-        complex = r2c(paint) / nbar (and the interlaced combination formed directly in Fourier space)."""
+        complex = r2c(paint) / nbar (and the interlaced combination formed directly in Fourier space).
+        x_pending=True (FFTPower's fused x pass and binning): where RealField._r2c_zy applies to a non-interlaced
+        mesh, the field is returned after the z and y passes only, with `_x_scale` = 1/nbar, the factor the x pass
+        still owes on top of 1/prod(Nmesh); a complete field has no `_x_scale`."""
         painted, N, W, W2 = self._paint_raw()
         attrs, nbar = self._attrs_for(N, W, W2)
-        if nbar <= 0:
+        c = painted._r2c_zy() if (x_pending and nbar > 0 and not self.interlaced) else None
+        if c is not None:
+            c._x_scale = 1.0 / nbar
+        elif nbar <= 0:
             real = painted[0] if self.interlaced else painted
             real[...] = 1
             c = real.r2c()
@@ -329,16 +335,16 @@ class CatalogMesh(MeshSource):
             self.logger.info("painted %d objects to mesh" % N)
         return c
 
-    def compute_complex_deferred(self, Nmesh=None):
+    def compute_complex_deferred(self, Nmesh=None, x_pending=False):
         """FFTPower fast path: (complex field WITHOUT the window compensation, name of the compensation the
         caller must still apply) when the compensation is the only action -- the power-binning kernel then
         applies it on the fly.  Falls back to (compute('complex', Nmesh=Nmesh), None) -- also whenever another
-        mesh size is asked for (the resampling of MeshSource.compute applies)."""
+        mesh size is asked for (the resampling of MeshSource.compute applies).  x_pending: see to_complex_field."""
         own = self._get_compensation() if self.compensated else []
         other_n = Nmesh is not None and any(numpy.ones(3, dtype='i8') * Nmesh != self.attrs['Nmesh'])
         if list(MeshSource.actions.fget(self)) or not own or other_n:
             return self.compute(mode='complex', Nmesh=Nmesh), None
-        c = self.to_complex_field()
+        c = self.to_complex_field(x_pending=x_pending)
         c.attrs.update(self.attrs)
         return c, own[0][1].__name__
 
