@@ -2,13 +2,16 @@
 Bispectrum benchmark: FFTBispectrum of a LogNormalCatalog of 1e7 objects (L = 1000 Mpc/h) with 32 shells up to the
 Nyquist wavenumber, painted to 256^3 in f8 and to 512^3 in f4.
 
-  python bench_bispectrum.py [--sizes 256f8,512f4] [--warmup 1]
+  python bench_bispectrum.py [--sizes 256f8,512f4] [--warmup 1] [--poles 0,2,4]
   torchrun --nproc-per-node N bench_bispectrum.py               (several GPUs, one process each)
 
 Prints one JSON line: the card and its power limit (read in the same run); per workload the wall time, the CUDA-event
 stage times (fill, c2r, triple sum, all-reduce), the c2r count and triangles evaluated; the triple-sum FLOPs over the
 H100 SXM data sheet's non-tensor FP64 rate (the products are formed in float64 for both precisions) and the fill bytes
 over its HBM3 bandwidth -- data-sheet bounds, not measured peaks; and the agreement with the float64 oracle at 64^3.
+With --poles, each workload also times a call with those multipoles (line of sight z) under "poles": wall time, stage
+times (the weighted fills are "fill_poles"), c2r count, weighted rows, and the peak device memory torch allocated during
+that call and during a plain call of the same workload.
 """
 import argparse
 import json
@@ -57,11 +60,47 @@ def fill_bytes(N, P, typestr, transforms_per_pass, fill_chunk):
     return cslab * (isz * (calls + transforms_per_pass) + 16 * transforms_per_pass)
 
 
+def _time_poles(mesh, dk, poles, comm, warmup):
+    """one timed FFTBispectrum call with multipoles: wall time, stage times, c2r count, weighted rows; and the peak
+    device memory allocated during it and during a plain call, both above what was allocated before the call"""
+    from nbodykit_b200 import _lib
+    from nbodykit_b200.algorithms import bispectrum as bs
+    from nbodykit_b200.lab import FFTBispectrum
+    for _ in range(warmup):
+        FFTBispectrum(mesh, dk=dk, poles=poles)
+    torch.cuda.synchronize()
+    _lib.profiler.start()
+    comm.barrier()
+    t0 = time.perf_counter()
+    r = FFTBispectrum(mesh, dk=dk, poles=poles)
+    torch.cuda.synchronize()
+    comm.barrier()
+    wall = time.perf_counter() - t0
+    stages = {k.replace("bispec_", ""): round(sum(v), 3) for k, v in _lib.profiler.stop().items()
+              if k.startswith("bispec_")}
+    nrow = len(bs.pole_triples(r.bispec.edges["k1"]))
+    c2r = int(r.attrs["transforms"])
+    del r
+    peak = {}
+    for name, kw in (("poles", dict(poles=poles)), ("plain", {})):
+        torch.cuda.synchronize()
+        torch.cuda.reset_peak_memory_stats()
+        base = torch.cuda.memory_allocated()
+        FFTBispectrum(mesh, dk=dk, **kw)
+        torch.cuda.synchronize()
+        peak[name] = round((torch.cuda.max_memory_allocated() - base) / 2 ** 30, 2)
+    return dict(poles=poles, seconds=round(wall, 4), stages_ms=stages, c2r=c2r,
+                weighted_rows=nrow * len([ell for ell in poles if ell > 0]), peak_gib=peak["poles"],
+                plain_peak_gib=peak["plain"])
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--sizes", default="256f8,512f4")
     ap.add_argument("--warmup", type=int, default=1)
+    ap.add_argument("--poles", default="", help="also time a call with these multipoles, e.g. 0,2,4")
     args = ap.parse_args()
+    poles = [int(v) for v in args.poles.split(",")] if args.poles else []
 
     from nbodykit_b200 import _lib
     from nbodykit_b200.algorithms import bispectrum as bs
@@ -105,6 +144,8 @@ def main():
             triple_sum_fp64_bound_fraction=round(flops / tsum_s / DATASHEET_FP64, 4),
             fill_bytes=fbytes, fill_tb_per_s=round(fbytes / fill_s / 1e12, 3),
             fill_hbm_bound_fraction=round(fbytes / fill_s / DATASHEET_HBM, 4))
+        if poles:
+            res["sizes"][size]["poles"] = _time_poles(mesh, dk, poles, comm, args.warmup)
         del mesh, r
     del src
 

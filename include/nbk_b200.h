@@ -443,6 +443,10 @@ int nbk_threeptcf(const double *ppos, const double *pw, const int64_t *chunk_fir
  *                k2edges_host (squared k edges): out[s][slab] = c * 1_S (complex of dtype) or, indicator != 0, the
  *                complex f8 indicator 1_S, s = 0 .. nshell - 1, out_stride complex elements apart.  A mode is in shell
  *                b - 1 when nbk_power_bin puts it in bin b at float32 coordinates; the k = 0 mode is in no shell.
+ *   fill_poles : the same pass writes, for the nell even multipoles ells_host[q] (0 .. 8, at most 5) and the same shells,
+ *                out[q nshell + s][slab] = c * L_ell(mu) * 1_S (complex of dtype), out_stride complex elements apart;
+ *                mu = k.los / |k| in float32 as nbk_power_bin forms it for a Python-number los (coordinate mode 4),
+ *                L_ell in float64, the product rounded once to dtype.
  *   triple_sum : fields holds nfield real fields of ncell values (dtype), field_stride elements apart; triples ntri
  *                device int triples (i, j, l) of slots < nfield.  Accumulates (device, zero first)
  *                out[t] += sum_x f_i f_j f_l, products and sums in float64. */
@@ -450,6 +454,9 @@ int nbk_bispec_max_shells(void);
 int nbk_bispec_fill(const void *cplx, int dtype, const int64_t *nmesh_host, const double *box_host, int layout, int64_t start,
                     int64_t count, const double *k2edges_host, int nedges, int shell0, int nshell, int indicator, void *out,
                     int64_t out_stride, void *stream);
+int nbk_bispec_fill_poles(const void *cplx, int dtype, const int64_t *nmesh_host, const double *box_host, int layout,
+                          int64_t start, int64_t count, const double *k2edges_host, int nedges, int shell0, int nshell,
+                          const double *los_host, const int *ells_host, int nell, void *out, int64_t out_stride, void *stream);
 int nbk_bispec_triple_sum(const void *fields, int dtype, int64_t field_stride, int nfield, int64_t ncell, const int *triples,
                           int64_t ntri, double *out, void *stream);
 

@@ -279,17 +279,6 @@ struct BinParams {
     double volume;
 };
 
-__device__ __forceinline__ double legendre(int ell, double x) {
-    if (ell == 0) return 1.0;
-    double p0 = 1.0, p1 = x;
-    for (int n = 1; n < ell; n++) {
-        double p2 = ((2 * n + 1) * x * p1 - n * p0) / (n + 1);
-        p0 = p1;
-        p1 = p2;
-    }
-    return p1;
-}
-
 template <typename T> struct Pair2;
 template <> struct Pair2<float> { typedef float2 type; };
 template <> struct Pair2<double> { typedef double2 type; };

@@ -1,6 +1,8 @@
 // FFT bispectrum estimator (algorithms/bispectrum.py: FFTBispectrum; DESIGN.md 4.14):
 //   nbk_bispec_fill       -- one read of the compressed Fourier slab writes c * 1_S or the f8 indicator 1_S for a
 //                            range of k shells (the inputs of the shell c2r transforms)
+//   nbk_bispec_fill_poles -- the same read writes c * L_ell(mu) * 1_S for a range of shells and several even ell (the
+//                            inputs of the multipole fields W^ell; mu = k.los / |k| in nbk_power_bin's float32 arithmetic)
 //   nbk_bispec_triple_sum -- sum_x f_i f_j f_l over resident real x-slab fields for a device list of slot triples
 //
 // Built with --fmad=false: the shell of a mode is decided by the float32 coordinate arithmetic of nbk_power_bin
@@ -12,6 +14,7 @@
 #define BS_TILE 64       // cells per shared-memory tile of the triple sum
 #define BS_TPT 4         // triples per thread of the triple sum
 #define BS_THREADS 256
+#define BS_MAX_ELL 5     // ell = 0, 2, 4, 6, 8: the most multipoles one fill_poles call writes
 
 struct FillParams {
     SlabGeom g;
@@ -59,6 +62,76 @@ k_bispec_fill(const typename Cplx<T>::type *__restrict__ c, FillParams P, void *
             z.y = 0;
             V2 *o = reinterpret_cast<V2 *>(out) + e;
             for (int s = 0; s < P.nshell; s++) o[s * P.ostride] = (s == local) ? v : z;
+        }
+    }
+}
+
+// k_bispec_fill's shell rule, also returning the mode's float32 coordinates: the shell of element e of the slab relative
+// to P.shell0 (-1: the k = 0 mode or outside every shell; values >= nshell are shells after the range).  k_bispec_fill
+// keeps its own copy so that its generated code stays as it was.
+__device__ __forceinline__ int fill_shell(const FillParams &P, int64_t e, float &kx, float &ky, float &kzv, float &k2) {
+    const SlabGeom &g = P.g;
+    const int kz = (int)(e % g.Nzc);
+    const int64_t row = e / g.Nzc;
+    const int i1 = (int)(row % g.D1), i0 = (int)(row / g.D1);
+    int jx, jy, jz;
+    slab_freqs(g, i0, i1, kz, jx, jy, jz);
+    // (0 + kx^2) + ky^2, then + kz^2, in float32 as nbk_power_bin forms it
+    kx = (float)jx * P.kf32[0];
+    ky = (float)jy * P.kf32[1];
+    kzv = (float)jz * P.kf32[2];
+    const float kp2 = kx * kx + ky * ky;
+    k2 = kp2 + kzv * kzv;
+    const int b = nbk_k2_bin(P.k2e, P.nedge, (double)k2, (double)sqrtf(k2), P.kmin, P.inv_dk, P.uniform);
+    int local = b - 1 - P.shell0;
+    if (b < 1 || b >= P.nedge || (jx == 0 && jy == 0 && jz == 0)) local = -1;
+    return local;
+}
+
+struct PoleParams {
+    float los32[3];                     // the line of sight rounded to float32, as nbk_power_bin's coordinate mode 4
+    int nell;
+    int ells[BS_MAX_ELL];
+};
+
+// One thread per mode of the slab (grid-stride), the shell as in k_bispec_fill.  Output (q, s) -- multipole ells[q],
+// shell shell0 + s -- starts (q nshell + s) ostride complex elements into `out` and holds c L_ell(mu) at the modes of
+// its shell, 0 elsewhere.  mu = ((kx l0 + ky l1) + kz l2) / sqrtf(k2) in float32 (nbk_power_bin, coordinate mode 4),
+// L_ell(mu) in float64, the product rounded once to the mesh precision.  L_ell is even for even ell, so the weighted
+// half spectrum stays Hermitian.
+template <typename T>
+__global__ void __launch_bounds__(BS_THREADS)
+k_bispec_fill_poles(const typename Cplx<T>::type *__restrict__ c, FillParams P, PoleParams L, void *__restrict__ out) {
+    typedef typename Cplx<T>::type V2;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < P.nelem; e += (int64_t)gridDim.x * blockDim.x) {
+        float kx, ky, kzv, k2;
+        const int local = fill_shell(P, e, kx, ky, kzv, k2);
+        const bool in = local >= 0 && local < P.nshell;
+        double mu = 0.0, re = 0.0, im = 0.0;
+        if (in) {
+            const float lp = kx * L.los32[0] + ky * L.los32[1];
+            mu = (double)((lp + kzv * L.los32[2]) / sqrtf(k2));
+            const V2 v = c[e];
+            re = (double)v.x;
+            im = (double)v.y;
+        }
+        V2 *o = reinterpret_cast<V2 *>(out) + e;
+        for (int q = 0; q < L.nell; q++) {
+            V2 w;
+            w.x = 0;
+            w.y = 0;
+            if (in) {
+                const double f = legendre(L.ells[q], mu);
+                w.x = (T)(re * f);
+                w.y = (T)(im * f);
+            }
+            V2 *oq = o + (int64_t)q * P.nshell * P.ostride;
+            for (int s = 0; s < P.nshell; s++) {
+                V2 z;
+                z.x = 0;
+                z.y = 0;
+                oq[s * P.ostride] = (s == local) ? w : z;
+            }
         }
     }
 }
@@ -111,16 +184,15 @@ k_bispec_triple_sum(const T *__restrict__ f, int64_t fstride, int R, int64_t nce
 
 extern "C" int nbk_bispec_max_shells(void) { return BS_MAX_SHELLS; }
 
-extern "C" int nbk_bispec_fill(const void *cplx, int dtype, const int64_t *nmesh_host, const double *box_host, int layout,
-                               int64_t start, int64_t count, const double *k2edges_host, int nedges, int shell0, int nshell,
-                               int indicator, void *out, int64_t out_stride, void *stream) {
+// the fill parameters of shells [shell0, shell0 + nshell) on this slab; nout output slabs out_stride apart
+static int make_fill(int dtype, const int64_t *nmesh_host, const double *box_host, int layout, int64_t start, int64_t count,
+                     const double *k2edges_host, int nedges, int shell0, int nshell, int nout, int64_t out_stride,
+                     FillParams &P) {
     NBK_CHECK_ARG(dtype == NBK_F4 || dtype == NBK_F8, "bispec_fill: bad dtype %d", dtype);
     NBK_CHECK_ARG((layout & NBK_LAYOUT_FULLZ) == 0, "bispec_fill: the field must be Hermitian-compressed");
     NBK_CHECK_ARG(nedges >= 2 && nedges <= BS_MAX_SHELLS + 1, "bispec_fill: %d edges (2 .. %d)", nedges, BS_MAX_SHELLS + 1);
     NBK_CHECK_ARG(shell0 >= 0 && nshell >= 0 && shell0 + nshell <= nedges - 1, "bispec_fill: shells [%d,+%d) of %d", shell0,
                   nshell, nedges - 1);
-    NBK_CHECK_ARG(out != nullptr && (indicator || cplx != nullptr), "bispec_fill: null field");
-    FillParams P;
     int rc = make_slab(nmesh_host, layout, start, count, 1, P.g);
     if (rc) return rc;
     const double TWO_PI = 6.283185307179586476925286766559;
@@ -137,8 +209,19 @@ extern "C" int nbk_bispec_fill(const void *cplx, int dtype, const int64_t *nmesh
     P.shell0 = shell0;
     P.nshell = nshell;
     P.nelem = (int64_t)P.g.count * P.g.D1 * P.g.Nzc;
-    NBK_CHECK_ARG(nshell <= 1 || out_stride >= P.nelem, "bispec_fill: output shells overlap");
+    NBK_CHECK_ARG(nout <= 1 || out_stride >= P.nelem, "bispec_fill: output shells overlap");
     P.ostride = out_stride;
+    return NBK_OK;
+}
+
+extern "C" int nbk_bispec_fill(const void *cplx, int dtype, const int64_t *nmesh_host, const double *box_host, int layout,
+                               int64_t start, int64_t count, const double *k2edges_host, int nedges, int shell0, int nshell,
+                               int indicator, void *out, int64_t out_stride, void *stream) {
+    FillParams P;
+    int rc = make_fill(dtype, nmesh_host, box_host, layout, start, count, k2edges_host, nedges, shell0, nshell, nshell,
+                       out_stride, P);
+    if (rc) return rc;
+    NBK_CHECK_ARG(out != nullptr && (indicator || cplx != nullptr), "bispec_fill: null field");
     if (P.nelem == 0 || nshell == 0) return NBK_OK;
     cudaStream_t s = (cudaStream_t)stream;
     const int grid = nbk_grid_for(P.nelem, BS_THREADS, 8);
@@ -148,6 +231,36 @@ extern "C" int nbk_bispec_fill(const void *cplx, int dtype, const int64_t *nmesh
         k_bispec_fill<float, false><<<grid, BS_THREADS, 0, s>>>((const float2 *)cplx, P, out);
     } else {
         k_bispec_fill<double, false><<<grid, BS_THREADS, 0, s>>>((const double2 *)cplx, P, out);
+    }
+    NBK_LAUNCHED();
+    return NBK_OK;
+}
+
+extern "C" int nbk_bispec_fill_poles(const void *cplx, int dtype, const int64_t *nmesh_host, const double *box_host,
+                                     int layout, int64_t start, int64_t count, const double *k2edges_host, int nedges,
+                                     int shell0, int nshell, const double *los_host, const int *ells_host, int nell, void *out,
+                                     int64_t out_stride, void *stream) {
+    NBK_CHECK_ARG(nell >= 0 && nell <= BS_MAX_ELL, "bispec_fill_poles: %d multipoles (0 .. %d)", nell, BS_MAX_ELL);
+    FillParams P;
+    int rc = make_fill(dtype, nmesh_host, box_host, layout, start, count, k2edges_host, nedges, shell0, nshell,
+                       nshell * nell, out_stride, P);
+    if (rc) return rc;
+    PoleParams L;
+    L.nell = nell;
+    for (int q = 0; q < nell; q++) {
+        NBK_CHECK_ARG(ells_host[q] >= 0 && ells_host[q] <= 8 && ells_host[q] % 2 == 0,
+                      "bispec_fill_poles: ell = %d (even, 0 .. 8: odd ell give an imaginary statistic)", ells_host[q]);
+        L.ells[q] = ells_host[q];
+    }
+    for (int d = 0; d < 3; d++) L.los32[d] = (float)los_host[d];
+    NBK_CHECK_ARG(out != nullptr && cplx != nullptr, "bispec_fill_poles: null field");
+    if (P.nelem == 0 || nshell == 0 || nell == 0) return NBK_OK;
+    cudaStream_t s = (cudaStream_t)stream;
+    const int grid = nbk_grid_for(P.nelem, BS_THREADS, 8);
+    if (dtype == NBK_F4) {
+        k_bispec_fill_poles<float><<<grid, BS_THREADS, 0, s>>>((const float2 *)cplx, P, L, out);
+    } else {
+        k_bispec_fill_poles<double><<<grid, BS_THREADS, 0, s>>>((const double2 *)cplx, P, L, out);
     }
     NBK_LAUNCHED();
     return NBK_OK;

@@ -1,4 +1,4 @@
-// Fourier-slab geometry and the |k| bin of a mode, shared by nbk_power_bin (binning.cu) and the bispectrum shells
+// Fourier-slab geometry, the |k| bin of a mode and the Legendre weights of mu, shared by nbk_power_bin (binning.cu) and the bispectrum shells
 // (bispectrum.cu), so that a shell of FFTBispectrum holds exactly the modes FFTPower puts in the same k bin.  Both
 // translation units are built with --fmad=false: the float32 coordinate arithmetic that feeds k2 is part of that contract.
 #pragma once
@@ -65,6 +65,19 @@ __device__ __forceinline__ int nbk_k2_bin(const double *__restrict__ k2edges, in
     while (b > 0 && k2d < k2edges[b - 1]) b--;
     while (b < nedge && k2d >= k2edges[b]) b++;
     return b;
+}
+
+// Legendre polynomial L_ell(x) in float64 by Bonnet's recurrence: the FFTPower multipole weights (nbk_power_bin) and
+// the weights of the bispectrum multipole fields (nbk_bispec_fill_poles)
+__device__ __forceinline__ double legendre(int ell, double x) {
+    if (ell == 0) return 1.0;
+    double p0 = 1.0, p1 = x;
+    for (int n = 1; n < ell; n++) {
+        double p2 = ((2 * n + 1) * x * p1 - n * p0) / (n + 1);
+        p0 = p1;
+        p1 = p2;
+    }
+    return p1;
 }
 
 // The last (x) pass of the forward transform fused with the FFTPower 1d auto-power binning (k_fft_x_bin in fft.cu,
