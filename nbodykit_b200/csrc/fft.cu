@@ -1512,11 +1512,14 @@ static int launch_lines_tma(const void *src, void *dst, void *const *peer_host, 
 // x pass fused with the FFTPower 1d auto-power binning (one rank: lines of N = 64 R strided by Ny*Nzc).  FFTPower keeps
 // only the binned sums, so the transformed field is never stored: the pass reads the z + y output once, writes nothing.
 // A tile runs the row-group FFTs and the radix-R combine of k_fft_lines_tma and scales each mode exactly as its store
-// does.  The scaled modes go back into the tile's R slots column by column ([b][64] per slot, the position XOR-swizzled
-// by b, so that the combine's writes and the binning's reads are both free of bank conflicts).  A warp then bins 32
-// consecutive j = jx >= 0 of one (ky, kz) column together with their mirrors -j, which have the same |k| and mu for a
-// line of sight along z.  |k| grows with j, so equal bins are contiguous runs of lanes, which a segmented shuffle
-// reduction folds into one shared-memory atomic per run; each CTA adds its sums to the global ones at the end.
+// does.  The combine reads its R slots into registers and frees them at once: the next tile's boxes are issued before
+// the radix-R DFT, so they land while this tile is transformed and binned.  Each thread then stages the power |X|^2 of
+// its modes in `stage` ([B][N/2 + 2] doubles, its own area, not the ring), adding the mirror -j's power onto j's in a
+// second pass (p_j + p_-j, no atomics).  A warp walks 32 consecutive j = jx >= 0 at a time along one (ky, kz) column,
+// whose coordinates, compensation and weight it forms once, and whose modes it keeps from a mu division each when the
+// column's smallest |k| already puts mu in [-1, 1); -j has the same |k| and mu as j for a line of sight along z.
+// |k| grows with j, so equal bins are contiguous runs of lanes, which a segmented shuffle reduction folds into one
+// shared-memory atomic per run; each CTA adds its sums to the global ones at the end.
 // The bin of a mode must be the one nbk_power_bin gives it (binning.cu is built with --fmad=false, this file is not), so
 // its arithmetic uses explicit round-to-nearest intrinsics throughout.
 // The ring set-up and refill repeat k_fft_lines_tma's on purpose: the same code behind a shared helper struct measured
@@ -1527,13 +1530,19 @@ k_fft_x_bin(const __grid_constant__ CUtensorMap tmap, const typename C2<T>::type
             int64_t n_tiles, T scale, int NS, const XBinArgs a) {
     typedef typename C2<T>::type C;
     constexpr int S = 64, N = S * R, SLOT = S * B, NW = NT / 32, IT = S * B / NT;
-    static_assert((S * B) % NT == 0 && B <= 32, "tile geometry");
+    // staged powers: row pitch SP = 2 (mod 16) doubles, so a half warp's phase stores (8 columns x 2 consecutive j) and
+    // the Nyquist reads (one column per lane) hit 16 distinct 8-byte bank pairs; the binning reads 32 consecutive j
+    constexpr int SP = N / 2 + 2;
+    // a warp bins IPW items of 32 j, JPW of them along one column before the next column
+    constexpr int IPW = B * R / NW, JPW = IPW < R ? IPW : R;
+    static_assert((S * B) % NT == 0 && B <= 32 && (B * R) % NW == 0 && IPW % JPW == 0 && R % JPW == 0, "tile geometry");
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     C *ring = reinterpret_cast<C *>(smem_raw);                 // [NS][64][B]
     C *twN = ring + (size_t)NS * SLOT;
     C *tw64 = twN + N;
     uint64_t *bars = reinterpret_cast<uint64_t *>(tw64 + S);   // [NS]
-    double *s_k2 = reinterpret_cast<double *>(bars + NS);      // [nedge]
+    double *stage = reinterpret_cast<double *>(bars + NS);     // [B][SP]: p_j + p_-j of column b at b * SP + j, j <= N/2
+    double *s_k2 = stage + B * SP;                             // [nedge]
     const int nedge = a.nedge, nkb = nedge + 1;
     double *s_x = s_k2 + nedge;                                // per k bin (mu bin 1): sum |k| w, sum P w, sum w
     double *s_p = s_x + nkb;
@@ -1571,7 +1580,7 @@ k_fft_x_bin(const __grid_constant__ CUtensorMap tmap, const typename C2<T>::type
         const int bvalid = (int)((n_inner - inner0) < B ? (n_inner - inner0) : B);
         const int g0 = it * R, base = g0 % NS;
         lines_tma_groups<T, R, B, NT>(ring, bars, NS, g0, tw64, (T)1);
-        // ---- radix-R combine, scaled as the store of k_fft_lines_tma scales, back into the slots by column
+        // ---- radix-R combine: the tile's slots -> registers, then the slots are refilled with the next tile's groups
         C v[IT][R];
 #pragma unroll
         for (int i = 0; i < IT; i++) {
@@ -1584,112 +1593,6 @@ k_fft_x_bin(const __grid_constant__ CUtensorMap tmap, const typename C2<T>::type
                 const C x = ring[(size_t)sj * SLOT + pos * B + b];
                 v[i][j] = j ? cmul(x, twN[j * k]) : x;
             }
-            dftR<R, C>(v[i]);
-#pragma unroll
-            for (int m = 0; m < R; m++) v[i][m] = C{v[i][m].x * scale, v[i][m].y * scale};
-        }
-        __syncthreads();
-#pragma unroll
-        for (int i = 0; i < IT; i++) {
-            const int w = tid + NT * i, b = w % B, k = w / B;
-#pragma unroll
-            for (int m = 0; m < R; m++) {
-                int sm = base + m;
-                if (sm >= NS) sm -= NS;
-                ring[(size_t)sm * SLOT + b * S + (k ^ b)] = v[i][m];
-            }
-        }
-        __syncthreads();
-        // ---- binning.  Mode K = jx mod N of column b sits in slot base + K / 64 at b * 64 + ((K % 64) ^ b).
-        // stats of mode j of column b, plus its mirror N - j when `pair`: k bin, mu bin, weight, weighted |k| and P
-        auto mode_stats = [&](int b, int j, bool pair, int &kb, int &dm, unsigned &cnt, double &xs, double &ps) {
-            const int inner = inner0 + b, iy = inner / Nzc, kz = inner - iy * Nzc;
-            const int jx = nbk_freq(j, N), jy = nbk_freq(iy, Ny), jz = nbk_freq(kz, Nz);
-            const float kx = __fmul_rn((float)jx, kfx), ky = __fmul_rn((float)jy, kfy), kzv = __fmul_rn((float)jz, kfz);
-            const float k2 = __fadd_rn(__fadd_rn(__fmul_rn(kx, kx), __fmul_rn(ky, ky)), __fmul_rn(kzv, kzv));
-            const float kn = __fsqrt_rn(k2);
-            const float mu = kn == 0.0f ? 0.0f : __fdiv_rn(__fmul_rn(kzv, a.losz32), kn);
-            kb = nbk_k2_bin(s_k2, nedge, (double)k2, (double)kn, a.kmin, a.inv_dk, a.uniform);
-            dm = (mu >= -1.0f ? 1 : 0) + (mu >= 1.0f ? 1 : 0);       // numpy.digitize(mu, [-1, 1])
-            const bool nonsing = jz > 0;                               // Hermitian weight: 1 on the kz = 0 / Nz/2 planes
-            cnt = (nonsing ? 2u : 1u) * (pair ? 2u : 1u);
-            xs = __dmul_rn((double)kn, (double)cnt);
-            int sl = base + (j >> 6);
-            if (sl >= NS) sl -= NS;
-            C c = ring[(size_t)sl * SLOT + b * S + ((j & 63) ^ b)];
-            double p = __dadd_rn(__dmul_rn((double)c.x, (double)c.x), __dmul_rn((double)c.y, (double)c.y));
-            if (pair) {
-                const int K = N - j;
-                sl = base + (K >> 6);
-                if (sl >= NS) sl -= NS;
-                c = ring[(size_t)sl * SLOT + b * S + ((K & 63) ^ b)];
-                p = __dadd_rn(p, __dadd_rn(__dmul_rn((double)c.x, (double)c.x), __dmul_rn((double)c.y, (double)c.y)));
-            }
-            double vol = a.volume;
-            if (a.ct0) vol = __dmul_rn(__dmul_rn(vol, __dmul_rn(a.ct0[j], a.ct1[iy])), a.ctz[kz]);
-            ps = (jx == 0 && jy == 0 && jz == 0) ? 0.0 : __dmul_rn(p, vol);     // the zero mode is cleared
-            if (nonsing) ps = __dmul_rn(ps, 2.0);
-        };
-        // modes outside mu bin 1 (mu == 1 on the kz axis, a rounding below -1) go straight to the global sums
-        auto add_global = [&](int key, unsigned cnt, double xs, double ps) {
-            atomicAdd(&a.nsum[key], (unsigned long long)cnt);
-            if (xs != 0.0) atomicAdd(&a.xsum[key], xs);
-            if (ps != 0.0) atomicAdd(&a.ysum[2 * key], ps);
-        };
-        for (int t = warp; t < B * R; t += NW) {
-            const int b = t / R, j = (t - b * R) * 32 + lane;      // j < N / 2: pairs (j, N - j), j = 0 alone
-            if (b >= bvalid) continue;
-            int kb, dm;
-            unsigned cnt;
-            double xs, ps;
-            mode_stats(b, j, j > 0, kb, dm, cnt, xs, ps);
-            int key = kb;
-            if (dm != 1) { add_global(kb * 3 + dm, cnt, xs, ps); key = -1; cnt = 0; xs = 0.0; ps = 0.0; }
-            // equal-key runs of lanes -> one atomic per run
-            const int prev = __shfl_up_sync(FULL, key, 1);
-            const bool head = (lane == 0) || (prev != key);
-            const unsigned heads = __ballot_sync(FULL, head);
-            if (heads == 1u) {
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) {
-                    cnt += __shfl_xor_sync(FULL, cnt, o);
-                    xs += __shfl_xor_sync(FULL, xs, o);
-                    ps += __shfl_xor_sync(FULL, ps, o);
-                }
-            } else if (heads != FULL) {
-                const int seg = __popc(heads & (FULL >> (31 - lane)));
-                const unsigned above = heads & ~((2u << lane) - 1u);
-                const int next = above ? (__ffs(above) - 1) : 32;
-                int maxrun = next - (31 - __clz(heads & ((2u << lane) - 1u)));
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) maxrun = max(maxrun, __shfl_xor_sync(FULL, maxrun, o));
-                for (int o = 1; o < maxrun; o <<= 1) {
-                    const int so = __shfl_down_sync(FULL, seg, o);
-                    const bool take = (lane + o < 32) && (so == seg);
-                    const unsigned c_o = __shfl_down_sync(FULL, cnt, o);
-                    const double x_o = __shfl_down_sync(FULL, xs, o);
-                    const double p_o = __shfl_down_sync(FULL, ps, o);
-                    if (take) { cnt += c_o; xs += x_o; ps += p_o; }
-                }
-            }
-            if (head && key >= 0) {
-                atomicAdd(&s_n[key], cnt);
-                if (xs != 0.0) atomicAdd(&s_x[key], xs);
-                if (ps != 0.0) atomicAdd(&s_p[key], ps);
-            }
-        }
-        // the Nyquist modes jx = -N/2 (no mirror), one lane per column
-        if (warp == NW - 1 && lane < bvalid) {
-            int kb, dm;
-            unsigned cnt;
-            double xs, ps;
-            mode_stats(lane, N / 2, false, kb, dm, cnt, xs, ps);
-            if (dm != 1) add_global(kb * 3 + dm, cnt, xs, ps);
-            else {
-                atomicAdd(&s_n[kb], cnt);
-                if (xs != 0.0) atomicAdd(&s_x[kb], xs);
-                if (ps != 0.0) atomicAdd(&s_p[kb], ps);
-            }
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic accesses to the slots before the next TMA writes
         __syncthreads();
@@ -1698,6 +1601,140 @@ k_fft_x_bin(const __grid_constant__ CUtensorMap tmap, const typename C2<T>::type
             if (upto > G) upto = G;
             for (; issued < upto; issued++) issue(issued);
         }
+        // ---- DFT, scaled as the store of k_fft_lines_tma scales; powers of modes K = k + 64 m <= N/2 to the stage,
+        // then those of K > N/2 added onto their mirror N - K
+        double pw[IT][R];
+#pragma unroll
+        for (int i = 0; i < IT; i++) {
+            const int w = tid + NT * i, b = w % B, k = w / B;
+            dftR<R, C>(v[i]);
+#pragma unroll
+            for (int m = 0; m < R; m++) {
+                const C c = C{v[i][m].x * scale, v[i][m].y * scale};
+                pw[i][m] = __dadd_rn(__dmul_rn((double)c.x, (double)c.x), __dmul_rn((double)c.y, (double)c.y));
+                const int K = k + S * m;
+                if (K <= N / 2) stage[b * SP + K] = pw[i][m];
+            }
+        }
+        __syncthreads();
+#pragma unroll
+        for (int i = 0; i < IT; i++) {
+            const int w = tid + NT * i, b = w % B, k = w / B;
+#pragma unroll
+            for (int m = R / 2; m < R; m++) {
+                const int K = k + S * m;
+                if (K > N / 2) stage[b * SP + N - K] = __dadd_rn(stage[b * SP + N - K], pw[i][m]);
+            }
+        }
+        __syncthreads();
+        // ---- binning.  What depends on the column b alone: its (ky, kz) coordinates, compensation and weight.
+        struct Col { int iy, kz; float ky2, kz2, kzl; bool nonsing, yz0, mu_in; unsigned w; double wd, cy, cz; };
+        auto column = [&](int b) {
+            Col c;
+            const int inner = inner0 + b;
+            c.iy = inner / Nzc;
+            c.kz = inner - c.iy * Nzc;
+            const int jy = nbk_freq(c.iy, Ny), jz = nbk_freq(c.kz, Nz);
+            const float ky = __fmul_rn((float)jy, kfy), kzv = __fmul_rn((float)jz, kfz);
+            c.ky2 = __fmul_rn(ky, ky);
+            c.kz2 = __fmul_rn(kzv, kzv);
+            c.kzl = __fmul_rn(kzv, a.losz32);
+            c.nonsing = jz > 0;                                        // Hermitian weight: 1 on the kz = 0 / Nz/2 planes
+            c.w = c.nonsing ? 2u : 1u;
+            c.wd = c.nonsing ? 2.0 : 1.0;
+            c.yz0 = jy == 0 && jz == 0;
+            // |k| of a mode is at least that of jx = 0 (each rounded step is monotone), so its |mu| = |kzl| / |k|
+            // rounded is at most that of jx = 0: when mu of jx = 0 lies in [-1, 1), every mode of the column is in mu bin 1
+            const float kn0 = __fsqrt_rn(__fadd_rn(__fadd_rn(0.0f, c.ky2), c.kz2));
+            const float mu0 = kn0 == 0.0f ? 0.0f : __fdiv_rn(c.kzl, kn0);
+            c.mu_in = kn0 != 0.0f && mu0 >= -1.0f && mu0 < 1.0f;
+            c.cy = a.ct0 ? a.ct1[c.iy] : 0.0;
+            c.cz = a.ct0 ? a.ctz[c.kz] : 0.0;
+            return c;
+        };
+        // stats of mode j of column b, its power p (with the mirror's when `pair`): k bin, mu bin, weight, weighted |k|, P
+        auto mode_stats = [&](const Col &c, int j, double p, bool pair, int &kb, int &dm, unsigned &cnt, double &xs,
+                              double &ps) {
+            const int jx = nbk_freq(j, N);
+            const float kx = __fmul_rn((float)jx, kfx);
+            const float k2 = __fadd_rn(__fadd_rn(__fmul_rn(kx, kx), c.ky2), c.kz2);
+            const float kn = __fsqrt_rn(k2);
+            kb = nbk_k2_bin(s_k2, nedge, (double)k2, (double)kn, a.kmin, a.inv_dk, a.uniform);
+            dm = 1;
+            if (!c.mu_in) {
+                const float mu = kn == 0.0f ? 0.0f : __fdiv_rn(c.kzl, kn);
+                dm = (mu >= -1.0f ? 1 : 0) + (mu >= 1.0f ? 1 : 0);   // numpy.digitize(mu, [-1, 1])
+            }
+            cnt = pair ? 2u * c.w : c.w;
+            xs = __dmul_rn((double)kn, pair ? 2.0 * c.wd : c.wd);
+            double vol = a.volume;
+            if (a.ct0) vol = __dmul_rn(__dmul_rn(vol, __dmul_rn(a.ct0[j], c.cy)), c.cz);
+            ps = (jx == 0 && c.yz0) ? 0.0 : __dmul_rn(p, vol);     // the zero mode is cleared
+            if (c.nonsing) ps = __dmul_rn(ps, 2.0);
+        };
+        // modes outside mu bin 1 (mu == 1 on the kz axis, a rounding below -1) go straight to the global sums
+        auto add_global = [&](int key, unsigned cnt, double xs, double ps) {
+            atomicAdd(&a.nsum[key], (unsigned long long)cnt);
+            if (xs != 0.0) atomicAdd(&a.xsum[key], xs);
+            if (ps != 0.0) atomicAdd(&a.ysum[2 * key], ps);
+        };
+        for (int t0 = warp * IPW; t0 < (warp + 1) * IPW; t0 += JPW) {
+            const int b = t0 / R;
+            if (b >= bvalid) break;
+            const Col col = column(b);
+            for (int jb = t0 - b * R; jb < t0 - b * R + JPW; jb++) {
+                const int j = jb * 32 + lane;                           // j < N / 2: pairs (j, N - j), j = 0 alone
+                int kb, dm;
+                unsigned cnt;
+                double xs, ps;
+                mode_stats(col, j, stage[b * SP + j], j > 0, kb, dm, cnt, xs, ps);
+                int key = kb;
+                if (dm != 1) { add_global(kb * 3 + dm, cnt, xs, ps); key = -1; cnt = 0; xs = 0.0; ps = 0.0; }
+                // equal-key runs of lanes -> one atomic per run
+                const int prev = __shfl_up_sync(FULL, key, 1);
+                const bool head = (lane == 0) || (prev != key);
+                const unsigned heads = __ballot_sync(FULL, head);
+                if (heads == 1u) {
+#pragma unroll
+                    for (int o = 16; o > 0; o >>= 1) {
+                        cnt += __shfl_xor_sync(FULL, cnt, o);
+                        xs += __shfl_xor_sync(FULL, xs, o);
+                        ps += __shfl_xor_sync(FULL, ps, o);
+                    }
+                } else if (heads != FULL) {
+                    // step o runs while some run is longer than o, i.e. o consecutive lanes are no heads; lane + o
+                    // is in this lane's run when none of lanes lane + 1 .. lane + o is a head
+                    unsigned more = ~heads;                             // lanes that continue a run
+                    for (int o = 1; more; o <<= 1) {
+                        const bool take = (lane + o < 32) && ((heads >> lane >> 1) & ((1u << o) - 1u)) == 0u;
+                        const unsigned c_o = __shfl_down_sync(FULL, cnt, o);
+                        const double x_o = __shfl_down_sync(FULL, xs, o);
+                        const double p_o = __shfl_down_sync(FULL, ps, o);
+                        if (take) { cnt += c_o; xs += x_o; ps += p_o; }
+                        more &= more >> o;                              // lanes starting o more continuing lanes
+                    }
+                }
+                if (head && key >= 0) {
+                    atomicAdd(&s_n[key], cnt);
+                    if (xs != 0.0) atomicAdd(&s_x[key], xs);
+                    if (ps != 0.0) atomicAdd(&s_p[key], ps);
+                }
+            }
+        }
+        // the Nyquist modes jx = -N/2 (no mirror), one lane per column
+        if (warp == NW - 1 && lane < bvalid) {
+            int kb, dm;
+            unsigned cnt;
+            double xs, ps;
+            mode_stats(column(lane), N / 2, stage[lane * SP + N / 2], false, kb, dm, cnt, xs, ps);
+            if (dm != 1) add_global(kb * 3 + dm, cnt, xs, ps);
+            else {
+                atomicAdd(&s_n[kb], cnt);
+                if (xs != 0.0) atomicAdd(&s_x[kb], xs);
+                if (ps != 0.0) atomicAdd(&s_p[kb], ps);
+            }
+        }
+        // the next tile's stage stores follow the CTA barriers of its row-group FFTs and its combine
     }
     __syncthreads();
     for (int i = tid; i < nkb; i += NT) {
@@ -1720,8 +1757,11 @@ static int launch_x_bin(void *cplx, double scale, const XBinArgs &a, cudaStream_
     const int R = N / 64;
     constexpr int B = 128 / (int)sizeof(C);
     const size_t cs = sizeof(C), slot = (size_t)64 * B * cs;
-    // as k_fft_lines_tma's ring, less the bytes of the edges and the accumulators (one slot at N = 1024)
-    const size_t fixed = (size_t)(N + 64) * cs + 26 * 8 + (size_t)a.nedge * 8 + (size_t)(a.nedge + 1) * 20 + 64;
+    // as k_fft_lines_tma's ring, less the staged powers (B (N/2 + 2) doubles: 4 slots at N = 1024) and the edges and
+    // accumulators (20 B per k bin + the f8 edges: close to 2 slots at N = 1024 with its N/2 default bins).  The slots are
+    // freed before the radix-R DFT, so R + 1 of them keep the next tile's boxes in flight through the DFT and binning.
+    const size_t fixed = (size_t)(N + 64) * cs + 26 * 8 + (size_t)B * (N / 2 + 2) * 8 + (size_t)a.nedge * 8 +
+                         (size_t)(a.nedge + 1) * 20 + 64;
     const int per_sm = tma_ctas_per_sm(R);
     const size_t budget = (size_t)(226 * 1024) / per_sm - 1024;
     if (budget < fixed + (size_t)(R + 1) * slot) return NBK_OK;     // too many bins for shared memory
