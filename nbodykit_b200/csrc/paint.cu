@@ -10,6 +10,7 @@
 // read-modify-write of spatially coherent catalogues.
 #include "common.cuh"
 #include <stdlib.h>
+#include <type_traits>
 
 template <int SUP> struct Window;
 
@@ -234,7 +235,10 @@ static int paint_impl(const void *pos, int pos_dtype, int64_t n, const void *mas
 //
 //   probe   k_bucket_probe    : samples neighbouring particle pairs: is the input spatially coherent (e.g. the
 //                               cell-sorted output of a mock generator)?  Picks the bucketing configuration ON THE
-//                               DEVICE (no host round trip): both configurations are launched, the other one exits.
+//                               DEVICE (no host round trip): all configurations are launched, the others exit.
+//                               Catalogues whose consecutive particles mostly share a tile take the RUN plan
+//                               (k_run_count / k_run_place, see there): runs are bucketed instead of 12-byte records and
+//                               the tile pass rebuilds each particle's record from its position.
 //   pass A  k_bucket_count    : every CTA owns contiguous particle chunks (aligned quads per thread, 16-byte loads) and
 //                               histograms the tile ids in a shared-memory WINDOW of tile indices (native
 //                               ATOMS.ADD.U32); one global atomic per (chunk, tile) reserves the chunk's share of the
@@ -462,6 +466,17 @@ __device__ __forceinline__ int make_record_pow2(const float *x, const TileGeom &
     return tile_from_cells(c, tg);
 }
 
+// the record of one particle and its tile (-1: outside the slab): what the scatter pass stores and the run plan's
+// tile pass rebuilds, bit for bit
+template <int SUP, typename PT>
+__device__ __forceinline__ int particle_record(const PT *x, const TileGeom &tg, const FastTile &ft, unsigned *rec) {
+    bool okp = false;
+    int t = -1;
+    if (sizeof(PT) == 4 && ft.pow2) t = make_record_pow2<SUP>(reinterpret_cast<const float *>(x), tg, ft, rec, okp);
+    if (!okp) t = make_record<SUP, PT>(x, tg, rec);
+    return t;
+}
+
 // Tile id of a particle.  float32 in-box positions take a float32 fast path: unless the fraction of
 // (x*scale + A) lies within the rounding margin of a cell boundary, floor() agrees with the exact f8 arithmetic;
 // everything else (near-boundary, outside the box, f8 positions) is recomputed in f8 (ok == false).  The id is
@@ -571,12 +586,14 @@ struct BucketPlan {          // one bucketing configuration (host side, by value
 };
 
 // Is the catalogue spatially coherent in array order?  256 threads sample neighbouring pairs (i, i+1): coherent pairs
-// lie within one plane of tiles of each other.  mode <- 1 (coherent) when >= 3/4 of the valid pairs are.
+// lie within one plane of tiles of each other.  mode <- 1 (coherent) when >= 3/4 of the valid pairs are.  The share of
+// pairs in the SAME tile estimates 1 - 1 / (mean run length): mode <- 2 (runs) when it is >= 2/3, i.e. runs of >= 3
+// particles on average, where bucketing runs moves fewer bytes than bucketing records (DESIGN.md 4.1).
 template <int SUP, typename PT>
 __global__ void __launch_bounds__(256)
-k_bucket_probe(const PT *__restrict__ pos, int64_t n, TileGeom tg, unsigned *__restrict__ hdr) {
-    __shared__ int s_ok, s_tot;
-    if (threadIdx.x == 0) { s_ok = 0; s_tot = 0; }
+k_bucket_probe(const PT *__restrict__ pos, int64_t n, TileGeom tg, int runs_ok, unsigned *__restrict__ hdr) {
+    __shared__ int s_ok, s_tot, s_eq;
+    if (threadIdx.x == 0) { s_ok = 0; s_tot = 0; s_eq = 0; }
     __syncthreads();
     const int plane = tg.nt[1] * tg.nt[2];
     int64_t j = (n > 1) ? (int64_t)((double)threadIdx.x / 256.0 * (double)(n - 1)) : 0;
@@ -588,10 +605,12 @@ k_bucket_probe(const PT *__restrict__ pos, int64_t n, TileGeom tg, unsigned *__r
             atomicAdd(&s_tot, 1);
             int d = ta / plane - tb / plane;
             if (d >= -1 && d <= 1) atomicAdd(&s_ok, 1);
+            if (ta == tb) atomicAdd(&s_eq, 1);
         }
     }
     __syncthreads();
-    if (threadIdx.x == 0) hdr[HDR_MODE] = (s_tot > 0 && 4 * s_ok >= 3 * s_tot) ? 1u : 0u;
+    if (threadIdx.x == 0)
+        hdr[HDR_MODE] = (runs_ok && s_tot > 0 && 3 * s_eq >= 2 * s_tot) ? 2u : (s_tot > 0 && 4 * s_ok >= 3 * s_tot) ? 1u : 0u;
 }
 
 // quad of this thread, straight from global memory
@@ -848,11 +867,7 @@ k_bucket_scatter(const PT *__restrict__ pos, const void *__restrict__ mass, int 
             for (int u = 0; u < 4; u++) {
                 r[u][0] = r[u][1] = r[u][2] = 0;
                 t[u] = -1;
-                if (u < nv) {
-                    bool okp = false;
-                    if (sizeof(PT) == 4 && ft.pow2) t[u] = make_record_pow2<SUP>(reinterpret_cast<const float *>(x[u]), tg, ft, r[u], okp);
-                    if (!okp) t[u] = make_record<SUP, PT>(x[u], tg, r[u]);
-                }
+                if (u < nv) t[u] = particle_record<SUP, PT>(x[u], tg, ft, r[u]);
                 const unsigned rel = (unsigned)(t[u] - lo);
                 k[u] = (t[u] >= 0 && rel < (unsigned)bp.W) ? (int)rel : -1;
                 anyout = anyout || (t[u] >= 0 && k[u] < 0);
@@ -911,6 +926,146 @@ k_bucket_scatter(const PT *__restrict__ pos, const void *__restrict__ mass, int 
                 }
             }
         });
+        __syncthreads();
+    }
+}
+
+// ---- run plan (mode 2).  A RUN is a maximal stretch of consecutive particles with the same tile inside one warp's
+// 128-particle slice of a round.  Entry = {first particle, tile << 7 | (length - 1)}; the runs of chunk c fill the
+// chunk's own region [c * chunk, ...) of the run list, so the list (one entry per particle at most) cannot overflow.
+#define RUN_TILE_BITS 25
+
+// pass A of the run plan: the count pass's chunks, window and exact tile ids, but one histogram count per RUN; writes
+// the runs and their number per chunk
+template <int SUP, typename PT>
+__global__ void __launch_bounds__(512, 2)
+k_run_count(const PT *__restrict__ pos, const void *__restrict__ mass, int mass_f4, int64_t n, TileGeom tg, FastTile ft,
+            unsigned *__restrict__ hdr, unsigned *__restrict__ cnt_w, unsigned *__restrict__ cnt_o,
+            unsigned *__restrict__ blk, int *__restrict__ win_lo, uint2 *__restrict__ runs, unsigned *__restrict__ run_n,
+            BucketPlan bp) {
+    if ((int)hdr[HDR_MODE] != bp.mode) return;
+    extern __shared__ __align__(128) unsigned char s_raw[];
+    unsigned *s_hist = reinterpret_cast<unsigned *>(s_raw);
+    __shared__ int s_lo;
+    __shared__ unsigned s_nrun;
+    const bool aligned = (reinterpret_cast<uintptr_t>(pos) & 15) == 0;
+    const unsigned lane = threadIdx.x & 31;
+    float mx = 0.f;
+    for (int c = blockIdx.x; c < bp.nchunks; c += gridDim.x) {
+        const int64_t b = (int64_t)c * bp.chunk;
+        const int64_t e = (b + bp.chunk < n) ? b + bp.chunk : n;
+        const int cn = e > b ? (int)(e - b) : 0;
+        const PT *cpos = pos + 3 * b;
+        uint2 *crun = runs + b;
+        for (int i = threadIdx.x; i < bp.W; i += blockDim.x) s_hist[i] = 0;
+        if (threadIdx.x == 0) s_nrun = 0;
+        __syncthreads();
+        const int lo = chunk_window_lo<SUP, PT>(cpos, cn, tg, bp.W, &s_lo);
+        if (threadIdx.x == 0) win_lo[c] = lo;
+        chunk_rounds<PT>(cpos, cn, aligned, [&](int j0, int nv, const PT (&x)[4][3]) {
+            int t[4];
+            quad_tiles<SUP, PT>(x, nv, tg, ft, t);
+            // boundaries: the slice's first particle and every tile change (t = -1 ends a run and starts none)
+            const int prev = __shfl_up_sync(0xffffffffu, t[3], 1);
+            bool bnd[4];
+            bnd[0] = lane == 0 || prev != t[0];
+#pragma unroll
+            for (int u = 1; u < 4; u++) bnd[u] = t[u] != t[u - 1];
+            unsigned B[4], H[4];
+#pragma unroll
+            for (int u = 0; u < 4; u++) {
+                B[u] = __ballot_sync(0xffffffffu, bnd[u]);
+                H[u] = __ballot_sync(0xffffffffu, bnd[u] && t[u] >= 0);
+            }
+            // first boundary after this lane's quad (slice position 4 * lane + u), 128 = end of the slice
+            const unsigned above = (B[0] | B[1] | B[2] | B[3]) & ~((2u << lane) - 1u);
+            int next = 128;
+            if (above) {
+                const int L = __ffs(above) - 1;
+                next = 4 * L + (((B[0] >> L) & 1u) ? 0 : ((B[1] >> L) & 1u) ? 1 : ((B[2] >> L) & 1u) ? 2 : 3);
+            }
+            int len[4];
+#pragma unroll
+            for (int u = 3; u >= 0; u--) {
+                const int p = 4 * (int)lane + u;
+                len[u] = next - p;
+                if (bnd[u]) next = p;
+            }
+            const unsigned lt = (1u << lane) - 1u;
+            unsigned rank = 0, tot = 0;
+#pragma unroll
+            for (int u = 0; u < 4; u++) { rank += __popc(H[u] & lt); tot += __popc(H[u]); }
+            unsigned base = 0;
+            if (lane == 0 && tot) base = atomicAdd(&s_nrun, tot);
+            rank += __shfl_sync(0xffffffffu, base, 0);
+            bool anyout = false;
+#pragma unroll
+            for (int u = 0; u < 4; u++) {
+                const bool head = (H[u] >> lane) & 1u;
+                const unsigned r = (unsigned)(t[u] - lo);
+                if (head) {
+                    if (r < (unsigned)bp.W) atomicAdd(&s_hist[r], 1u);
+                    else anyout = true;
+                    crun[rank++] = make_uint2((unsigned)(b + j0 + u), ((unsigned)t[u] << 7) | (unsigned)(len[u] - 1));
+                }
+            }
+            if (__any_sync(0xffffffffu, anyout)) {
+#pragma unroll
+                for (int u = 0; u < 4; u++)
+                    warp_claim(cnt_o, t[u], ((H[u] >> lane) & 1u) && (unsigned)(t[u] - lo) >= (unsigned)bp.W);
+            }
+            if (mass) {
+#pragma unroll
+                for (int u = 0; u < 4; u++)
+                    if (t[u] >= 0) mx = fmaxf(mx, fabsf((float)load_mass(mass, mass_f4, b + j0 + u)) * 1.0000001f);
+            }
+        });
+        __syncthreads();
+        unsigned *row = blk + (size_t)c * bp.W;
+        for (int i = threadIdx.x; i < bp.W; i += blockDim.x) {
+            const unsigned h = s_hist[i];
+            row[i] = h ? atomicAdd(&cnt_w[lo + i], h) : 0u;
+        }
+        if (threadIdx.x == 0) run_n[c] = s_nrun;
+        __syncthreads();
+    }
+    if (mass) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+        if ((threadIdx.x & 31) == 0 && mx > 0.f) atomicMax(&hdr[HDR_ABSMAX], __float_as_uint(mx));
+    }
+}
+
+// pass C of the run plan: reads no positions; claims one bucket slot per run of the chunk (as k_bucket_scatter claims
+// one per particle) and stores the run's index in the run list there
+__global__ void __launch_bounds__(512)
+k_run_place(const uint2 *__restrict__ runs, const unsigned *__restrict__ run_n, int ntiles, const unsigned *__restrict__ hdr,
+            const unsigned *__restrict__ offsets, const unsigned *__restrict__ cnt_w, unsigned *__restrict__ cur_o,
+            const unsigned *__restrict__ blk, const int *__restrict__ win_lo, unsigned *__restrict__ bucket, BucketPlan bp) {
+    if ((int)hdr[HDR_MODE] != bp.mode) return;
+    extern __shared__ __align__(128) unsigned char s_raw[];
+    unsigned *s_cur = reinterpret_cast<unsigned *>(s_raw);
+    for (int c = blockIdx.x; c < bp.nchunks; c += gridDim.x) {
+        const int lo = win_lo[c];
+        const unsigned *row = blk + (size_t)c * bp.W;
+        const int wn = min(bp.W, ntiles - lo);
+        for (int i = threadIdx.x; i < wn; i += blockDim.x) s_cur[i] = offsets[lo + i] + row[i];
+        __syncthreads();
+        const unsigned nr = run_n[c];
+        const unsigned r0 = (unsigned)((int64_t)c * bp.chunk);
+        for (unsigned i0 = 0; i0 < nr; i0 += blockDim.x) {
+            const unsigned i = i0 + threadIdx.x;
+            const bool valid = i < nr;
+            const int t = valid ? (int)(runs[r0 + i].y >> 7) : -1;
+            const unsigned k = (unsigned)(t - lo);
+            const bool out = valid && k >= (unsigned)bp.W;
+            unsigned slot = (valid && !out) ? atomicAdd(&s_cur[k], 1u) : 0u;
+            if (__any_sync(0xffffffffu, out)) {
+                const unsigned so = warp_claim(cur_o, t, out);
+                if (out) slot = offsets[t] + cnt_w[t] + so;
+            }
+            if (valid) bucket[slot] = r0 + i;
+        }
         __syncthreads();
     }
 }
@@ -1023,11 +1178,17 @@ __host__ __device__ constexpr int tile_plane_pitch(int sup, int flush, int R, in
 //          warp, no CTA barrier) is almost never a wait.  Two CTA barriers per tile.  Tiles on the mesh boundary take
 //          a generic per-cell path (and wait in place where their add set does not fit the stash).
 // FLUSH 1: TMA bulk reduce-add, one row per op, into an existing mesh (hold=True)
-template <int SUP, typename MT, typename FT, bool SHIFTED, int FLUSH>
+// PT void: the record plans -- recs = 12-byte records, smass = their masses in bucket order.  PT float / double: the run
+// plan -- recs = run indices, runs = the run list, pos and smass = the catalogue's positions and masses; the records are
+// rebuilt from the positions (particle_record, bit for bit the scatter pass's), so the mesh is the record plans' mesh.
+template <int SUP, typename MT, typename FT, bool SHIFTED, int FLUSH, typename PT>
 __global__ void __launch_bounds__(256, FLUSH == 0 ? 4 : 1)
 k_tile_paint(const unsigned *__restrict__ recs, const MT *__restrict__ smass, TileGeom tg,
              const unsigned *__restrict__ offsets, unsigned *__restrict__ hdr, unsigned *__restrict__ flags,
-             unsigned epoch, FT *__restrict__ mesh, unsigned *__restrict__ d_off, FT *__restrict__ d_val, unsigned d_cap) {
+             unsigned epoch, FT *__restrict__ mesh, unsigned *__restrict__ d_off, FT *__restrict__ d_val, unsigned d_cap,
+             const uint2 *__restrict__ runs, const PT *__restrict__ pos, FastTile ft) {
+    constexpr bool RUNS = !std::is_void<PT>::value;
+    if ((hdr[HDR_MODE] == 2u) != RUNS) return;
     extern __shared__ __align__(16) unsigned s_all[];
     constexpr int R = TILE + SUP - 1 + (SHIFTED ? 1 : 0);   // == tg.R
     // row pitch in cells: the TMA write-back needs rows that start 16-byte aligned, the ordered one 8-byte cell pairs
@@ -1073,27 +1234,9 @@ k_tile_paint(const unsigned *__restrict__ recs, const MT *__restrict__ smass, Ti
                      "@p red.shared.add.u32 [%2], 1;\n"
                      "}\n" :: "r"(addr), "r"(q), "r"(addr + HIOFF) : "memory");
     };
-    // deposits of the records [b, e) of one bucket into the accumulator (HM: the catalogue carries masses)
-    auto accumulate_t = [&](unsigned b, unsigned e, auto hm_tag) {
-        constexpr bool HM = decltype(hm_tag)::value;
-        // thread p takes records p, p + NT, ... (coalesced)
-        const unsigned cnt = e - b;
-        unsigned idx = threadIdx.x;
-        unsigned rn[3] = {0, 0, 0};
-        MT mn = (MT)1;
-        if (idx < cnt) {
-            const unsigned *rp = recs + 3 * (size_t)(b + idx);
-            rn[0] = rp[0]; rn[1] = rp[1]; rn[2] = rp[2];
-            if (HM) mn = smass[b + idx];
-        }
-        for (; idx < cnt; idx += NT) {
-            const unsigned r0 = rn[0], r1 = rn[1], r2 = rn[2];
-            const MT mcur = mn;
-            if (idx + NT < cnt) {                            // next round's record is requested before the deposits
-                const unsigned *rp = recs + 3 * (size_t)(b + idx + NT);
-                rn[0] = rp[0]; rn[1] = rp[1]; rn[2] = rp[2];
-                if (HM) mn = smass[b + idx + NT];
-            }
+    // deposits of one record into the accumulator (HM: the catalogue carries masses)
+    auto deposit_record = [&](unsigned r0, unsigned r1, unsigned r2, MT mcur, auto hm_tag) {
+            constexpr bool HM = decltype(hm_tag)::value;
             unsigned u[3] = {r0 << 4, r1 << 4, r2 << 4};
             int l[3] = {(int)(r0 >> 28), (int)(r1 >> 28), (int)(r2 >> 28)};
             double w[3][SUP];
@@ -1140,11 +1283,99 @@ k_tile_paint(const unsigned *__restrict__ recs, const MT *__restrict__ smass, Ti
                             fixed_add(s_lo, s_hi, base0 + rx * PS + ry * RP + rz, __double2ll_rn(wxy * wz[rz]));
                     }
             }
+    };
+    // deposits of the records [b, e) of one bucket
+    auto accumulate_recs = [&](unsigned b, unsigned e, auto hm_tag) {
+        constexpr bool HM = decltype(hm_tag)::value;
+        // thread p takes records p, p + NT, ... (coalesced)
+        const unsigned cnt = e - b;
+        unsigned idx = threadIdx.x;
+        unsigned rn[3] = {0, 0, 0};
+        MT mn = (MT)1;
+        if (idx < cnt) {
+            const unsigned *rp = recs + 3 * (size_t)(b + idx);
+            rn[0] = rp[0]; rn[1] = rp[1]; rn[2] = rp[2];
+            if (HM) mn = smass[b + idx];
+        }
+        for (; idx < cnt; idx += NT) {
+            const unsigned r0 = rn[0], r1 = rn[1], r2 = rn[2];
+            const MT mcur = mn;
+            if (idx + NT < cnt) {                            // next round's record is requested before the deposits
+                const unsigned *rp = recs + 3 * (size_t)(b + idx + NT);
+                rn[0] = rp[0]; rn[1] = rp[1]; rn[2] = rp[2];
+                if (HM) mn = smass[b + idx + NT];
+            }
+            deposit_record(r0, r1, r2, mcur, hm_tag);
+        }
+    };
+    // deposits of the particles of the runs [b, e) of one bucket.  Warp w takes the runs b + 32 (w + 8 k) + lane (the
+    // next 32 are requested before these are painted); over the particles of its 32 runs (exclusive scan of the lengths)
+    // lane q takes particles q, q + 32, ...: the runs that start in a window of 32 particles form a bit mask (one
+    // REDUX.OR), so the run of each lane is a popcount away, and consecutive lanes read consecutive particles of a run.
+    auto accumulate_runs = [&](unsigned b, unsigned e, auto hm_tag) {
+        if constexpr (RUNS) {
+            constexpr bool HM = decltype(hm_tag)::value;
+            unsigned eb = b + 32 * wid;
+            uint2 rnext = make_uint2(0u, 0u);
+            if (eb + lane < e) rnext = runs[recs[eb + lane]];
+            for (; eb < e; eb += NT) {
+                const bool valid = eb + lane < e;
+                const unsigned len = valid ? (rnext.y & 127u) + 1u : 0u;
+                const unsigned st = rnext.x;
+                if (eb + NT + lane < e) rnext = runs[recs[eb + NT + lane]];
+                unsigned inc = len;
+#pragma unroll
+                for (int o = 1; o < 32; o <<= 1) {
+                    const unsigned v = __shfl_up_sync(0xffffffffu, inc, o);
+                    if ((int)lane >= o) inc += v;
+                }
+                const unsigned tot = __shfl_sync(0xffffffffu, inc, 31);
+                const unsigned exc = inc - len;
+                const unsigned base = st - exc;          // particle index = base + q for the q of this lane's run
+                unsigned before = 0;                     // runs that start before the current window
+                // particle index of this lane in the window [q0, q0 + 32); windows are taken in order; all lanes call
+                auto particle = [&](unsigned q0) -> unsigned {
+                    const unsigned m = __reduce_or_sync(0xffffffffu, (len && exc - q0 < 32u) ? 1u << (exc - q0) : 0u);
+                    const int j = (int)before + __popc(m & ((2u << lane) - 1u)) - 1;
+                    before += __popc(m);
+                    return __shfl_sync(0xffffffffu, base, j & 31) + q0 + lane;
+                };
+                PT xn[3] = {(PT)0, (PT)0, (PT)0};
+                MT mn = (MT)1;
+                {
+                    const unsigned i = particle(0);
+                    if (lane < tot) {
+                        xn[0] = pos[3 * (size_t)i]; xn[1] = pos[3 * (size_t)i + 1]; xn[2] = pos[3 * (size_t)i + 2];
+                        if (HM) mn = smass[i];
+                    }
+                }
+                for (unsigned q0 = 0; q0 < tot; q0 += 32) {
+                    const PT x[3] = {xn[0], xn[1], xn[2]};
+                    const MT mcur = mn;
+                    if (q0 + 32 < tot) {                     // the next particle is requested before the deposits
+                        const unsigned i = particle(q0 + 32);
+                        if (q0 + 32 + lane < tot) {
+                            xn[0] = pos[3 * (size_t)i]; xn[1] = pos[3 * (size_t)i + 1]; xn[2] = pos[3 * (size_t)i + 2];
+                            if (HM) mn = smass[i];
+                        }
+                    }
+                    if (q0 + lane < tot) {
+                        unsigned r[3];
+                        particle_record<SUP, PT>(x, tg, ft, r);
+                        deposit_record(r[0], r[1], r[2], mcur, hm_tag);
+                    }
+                }
+            }
         }
     };
     auto accumulate = [&](unsigned b, unsigned e) {
-        if (smass) accumulate_t(b, e, BoolTag<true>());
-        else accumulate_t(b, e, BoolTag<false>());
+        if constexpr (RUNS) {
+            if (smass) accumulate_runs(b, e, BoolTag<true>());
+            else accumulate_runs(b, e, BoolTag<false>());
+        } else {
+            if (smass) accumulate_recs(b, e, BoolTag<true>());
+            else accumulate_recs(b, e, BoolTag<false>());
+        }
     };
 
     if (FLUSH == 1) {
@@ -1535,10 +1766,11 @@ extern "C" int64_t nbk_paint_tiled_workspace(int64_t n, int pos_dtype, int mass_
     bytes += 5 * align256(sizeof(unsigned) * (nt + 1));  // cnt_w, cnt_o, offsets, cur_o, flags
     bytes += align256(sizeof(unsigned) * ((size_t)(nt + 4095) / 4096 + 1));     // segment totals of the offset scan
     bytes += align256(sizeof(int) * NBK_CHUNKS_COHERENT);                // window start per chunk
+    bytes += align256(sizeof(unsigned) * NBK_CHUNKS_COHERENT);           // runs per chunk (run plan)
     int64_t wc = nt < NBK_WIN_COHERENT ? nt : NBK_WIN_COHERENT, ws = nt < NBK_BLK_SMEM / 4 ? nt : NBK_BLK_SMEM / 4;
     int64_t blk = wc * NBK_CHUNKS_COHERENT > ws * NBK_CHUNKS_SCATTERED ? wc * NBK_CHUNKS_COHERENT : ws * NBK_CHUNKS_SCATTERED;
     bytes += align256(sizeof(unsigned) * (size_t)blk);                   // per-chunk bucket shares
-    bytes += align256((size_t)n * 12);                                   // 12-byte records
+    bytes += align256((size_t)n * 12);                                   // 12-byte records | run list (8 B) + run buckets (4 B)
     if (mass_dtype) bytes += align256((size_t)n * (mass_dtype == NBK_F4 ? 4 : 8));
     bytes += 2 * align256((size_t)nbk_defer_cap(nt) * 8);                // deferred halo adds: offsets (u32) and values (<= f8)
     return (int64_t)bytes;
@@ -1563,6 +1795,7 @@ static int run_tiled(const void *pos, const void *mass, int64_t n, const PaintGe
     unsigned *flags = (unsigned *)w; w += tb;
     unsigned *seg_tot = (unsigned *)w; w += align256(sizeof(unsigned) * ((size_t)(tg.ntiles + 4095) / 4096 + 1));   // scan: segment totals
     int *win_lo = (int *)w; w += align256(sizeof(int) * NBK_CHUNKS_COHERENT);
+    unsigned *run_n = (unsigned *)w; w += align256(sizeof(unsigned) * NBK_CHUNKS_COHERENT);
     BucketPlan coh, sca;
     int th_c, th_s;
     size_t sm_c, sm_s;
@@ -1573,6 +1806,8 @@ static int run_tiled(const void *pos, const void *mass, int64_t n, const PaintGe
         w += align256(sizeof(unsigned) * (a > b ? a : b));
     }
     unsigned *recs = (unsigned *)w; w += align256((size_t)n * 12);
+    uint2 *runs = reinterpret_cast<uint2 *>(recs);           // run plan: the run list and its buckets alias the records
+    unsigned *rbucket = recs + 2 * (size_t)n;
     MT *smass = mass ? (MT *)w : nullptr;
     if (mass) w += align256((size_t)n * sizeof(MT));
     // NBK_PAINT_DEFER_CAP: smaller list (tests the overflow path)
@@ -1584,17 +1819,24 @@ static int run_tiled(const void *pos, const void *mass, int64_t n, const PaintGe
     unsigned *d_off = (unsigned *)w; w += align256((size_t)nbk_defer_cap(tg.ntiles) * 8);
     FT *d_val = (FT *)w; w += align256((size_t)nbk_defer_cap(tg.ntiles) * 8);
     const int mass_f4 = sizeof(MT) == 4;
+    // The run plan packs the tile id into RUN_TILE_BITS bits.  Its tile pass rebuilds every record, once per mesh: the
+    // probe picks it for one NNB / CIC mesh, where that costs less than the record stream saves (DESIGN.md 4.1); TSC /
+    // PCS and the interlaced pair keep the record plans unless NBK_PAINT_BUCKET=runs forces it.
+    const int runs_ok = tg.ntiles <= (1 << RUN_TILE_BITS);
+    const int runs_auto = runs_ok && SUP <= 2 && mesh2 == nullptr;
     int force_mode;
     {
-        const char *e = getenv("NBK_PAINT_BUCKET");      // "coherent" / "scattered" force the configuration the probe picks
-        force_mode = (e && e[0] == 'c') ? 1 : (e && e[0] == 's') ? 0 : -1;
+        const char *e = getenv("NBK_PAINT_BUCKET");      // "coherent" / "scattered" / "runs" force the configuration the probe picks
+        force_mode = (e && e[0] == 'c') ? 1 : (e && e[0] == 's') ? 0 : (e && e[0] == 'r') ? 2 : -1;
     }
+    NBK_CHECK_ARG(force_mode != 2 || runs_ok, "paint_tiled: NBK_PAINT_BUCKET=runs needs at most 2^%d tiles", RUN_TILE_BITS);
+    const bool runs_on = force_mode == 2 || (force_mode < 0 && runs_auto);     // the run kernels are launched
     NBK_CUDA(cudaMemsetAsync(work, 0, 256 + 2 * tb, s));   // header, cnt_w, cnt_o
     if (force_mode >= 0) {
         unsigned m = (unsigned)force_mode;
         NBK_CUDA(cudaMemcpyAsync(&hdr[HDR_MODE], &m, sizeof(unsigned), cudaMemcpyHostToDevice, s));
     } else {
-        k_bucket_probe<SUP, PT><<<1, 256, 0, s>>>((const PT *)pos, n, tg, hdr);
+        k_bucket_probe<SUP, PT><<<1, 256, 0, s>>>((const PT *)pos, n, tg, runs_auto, hdr);
         NBK_LAUNCHED();
     }
     // Coherent plan: every resident CTA gets the same number of chunks in BOTH passes (their occupancies differ:
@@ -1629,6 +1871,24 @@ static int run_tiled(const void *pos, const void *mass, int64_t n, const PaintGe
     } while (0)
     // (the plan is the LAST kernel argument of both passes so that one macro serves them)
     LAUNCH_BUCKET(k_bucket_count, grid_c, sm_cnt, (const PT *)pos, mass, mass_f4, n, tg, ft, hdr, cnt_w, cnt_o, blk, win_lo);
+    // run plan: the coherent plan's chunks and window
+    BucketPlan rp = coh;
+    rp.mode = 2;
+    rp.wstage = 0;
+    const size_t sm_run = (size_t)coh.W * 4;
+    int grid_rc = 1, grid_rp = 1;
+    if (runs_on) {
+        NBK_CUDA(cudaFuncSetAttribute(k_run_count<SUP, PT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_run));
+        NBK_CUDA(cudaFuncSetAttribute(k_run_place, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_run));
+        int occ_rc = 1, occ_rp = 1;
+        NBK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_rc, k_run_count<SUP, PT>, 512, sm_run));
+        NBK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_rp, k_run_place, 512, sm_run));
+        grid_rc = rp.nchunks < max(occ_rc, 1) * NBK_SM_COUNT ? rp.nchunks : max(occ_rc, 1) * NBK_SM_COUNT;
+        grid_rp = rp.nchunks < max(occ_rp, 1) * NBK_SM_COUNT ? rp.nchunks : max(occ_rp, 1) * NBK_SM_COUNT;
+        k_run_count<SUP, PT><<<grid_rc, 512, sm_run, s>>>((const PT *)pos, mass, mass_f4, n, tg, ft, hdr, cnt_w, cnt_o, blk,
+                                                         win_lo, runs, run_n, rp);
+        NBK_LAUNCHED();
+    }
     {
         const int nseg = (tg.ntiles + 4095) / 4096;
         k_tile_scan_totals<<<nseg, 1024, 0, s>>>(cnt_w, cnt_o, seg_tot, tg.ntiles);
@@ -1639,22 +1899,33 @@ static int run_tiled(const void *pos, const void *mass, int64_t n, const PaintGe
     LAUNCH_BUCKET(k_bucket_scatter, grid_cs, sm_c, (const PT *)pos, mass, mass_f4, n, tg, ft, hdr, offsets, cnt_w, cur_o, blk, win_lo, recs,
                   (void *)smass);
 #undef LAUNCH_BUCKET
-    // the region edge depends on the mesh being painted (one more cell for the half-cell shifted one); tile ids do not
-#define LAUNCH_TP(SH, FL, MESHP, EPOCH)                                                                                \
+    if (runs_on) {
+        k_run_place<<<grid_rp, 512, sm_run, s>>>(runs, run_n, tg.ntiles, hdr, offsets, cnt_w, cur_o, blk, win_lo, rbucket, rp);
+        NBK_LAUNCHED();
+    }
+    // the region edge depends on the mesh being painted (one more cell for the half-cell shifted one); tile ids do not.
+    // Both sources are launched (the one the probe did not pick exits at once), then one pass adds the deferred sets.
+#define LAUNCH_TP1(SH, FL, MESHP, EPOCH, SRC, RECS, MASS)                                                              \
     do {                                                                                                              \
-        const int Rr = TILE + SUP - 1 + ((SH) ? 1 : 0), RPr = (FL) == 0 ? ((Rr + 1) & ~1) : ((Rr + 3) & ~3);                       \
+        const int Rr = TILE + SUP - 1 + ((SH) ? 1 : 0), RPr = (FL) == 0 ? ((Rr + 1) & ~1) : ((Rr + 3) & ~3);         \
         size_t smem = (size_t)((2 * Rr * tile_plane_pitch(SUP, FL, Rr, RPr) + 3) & ~3) * sizeof(unsigned);            \
         if ((FL) == 0) smem += (size_t)(Rr * Rr * Rr - TILE * TILE * TILE) * (sizeof(FT) + sizeof(unsigned));        \
-        NBK_CUDA(cudaFuncSetAttribute(k_tile_paint<SUP, MT, FT, SH, FL>, cudaFuncAttributeMaxDynamicSharedMemorySize,  \
+        NBK_CUDA(cudaFuncSetAttribute(k_tile_paint<SUP, MT, FT, SH, FL, SRC>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
                                       (int)smem));                                                                    \
         int per_sm = 1;                                                                                               \
-        NBK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_tile_paint<SUP, MT, FT, SH, FL>, 256, smem)); \
+        NBK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_tile_paint<SUP, MT, FT, SH, FL, SRC>, 256, smem)); \
         if (per_sm < 1) per_sm = 1;                                                                                   \
         int grid = NBK_SM_COUNT * per_sm;                                                                             \
         if (grid > tg.ntiles) grid = tg.ntiles;                                                                       \
-        k_tile_paint<SUP, MT, FT, SH, FL><<<grid, 256, smem, s>>>(recs, smass, tg, offsets, hdr, flags, EPOCH,         \
-                                                                  (FT *)(MESHP), d_off, d_val, d_cap);                \
+        k_tile_paint<SUP, MT, FT, SH, FL, SRC><<<grid, 256, smem, s>>>(RECS, MASS, tg, offsets, hdr, flags, EPOCH,    \
+                                                                       (FT *)(MESHP), d_off, d_val, d_cap, runs,      \
+                                                                       (const SRC *)pos, ft);                        \
         NBK_LAUNCHED();                                                                                               \
+    } while (0)
+#define LAUNCH_TP(SH, FL, MESHP, EPOCH)                                                                                \
+    do {                                                                                                              \
+        LAUNCH_TP1(SH, FL, MESHP, EPOCH, void, recs, smass);                                                         \
+        if (runs_on) LAUNCH_TP1(SH, FL, MESHP, EPOCH, PT, rbucket, (const MT *)mass);                                \
         if ((FL) == 0) {                                                                                              \
             k_apply_deferred<FT><<<NBK_SM_COUNT * 4, 256, 0, s>>>(hdr, d_off, d_val, d_cap, (FT *)(MESHP));           \
             NBK_LAUNCHED();                                                                                           \
@@ -1667,6 +1938,7 @@ static int run_tiled(const void *pos, const void *mass, int64_t n, const PaintGe
         NBK_CUDA(cudaMemsetAsync(&hdr[HDR_DEFER], 0, sizeof(unsigned), s));
         if (clear) LAUNCH_TP(true, 0, mesh2, 2u); else LAUNCH_TP(true, 1, mesh2, 2u);
     }
+#undef LAUNCH_TP1
 #undef LAUNCH_TP
     return NBK_OK;
 }
