@@ -447,6 +447,9 @@ int nbk_threeptcf(const double *ppos, const double *pw, const int64_t *chunk_fir
  *                out[q nshell + s][slab] = c * L_ell(mu) * 1_S (complex of dtype), out_stride complex elements apart;
  *                mu = k.los / |k| in float32 as nbk_power_bin forms it for a Python-number los (coordinate mode 4),
  *                L_ell in float64, the product rounded once to dtype.
+ *   fill_cross : the same pass over two slabs cplx, cplx2 of the same layout and dtype writes, for the same shells,
+ *                out[s][slab] = scale * c * conj(c2) * 1_S as complex f8 (the product formed in float64), out_stride
+ *                complex elements apart.
  *   triple_sum : fields holds nfield real fields of ncell values (dtype), field_stride elements apart; triples ntri
  *                device int triples (i, j, l) of slots < nfield.  Accumulates (device, zero first)
  *                out[t] += sum_x f_i f_j f_l, products and sums in float64. */
@@ -457,6 +460,9 @@ int nbk_bispec_fill(const void *cplx, int dtype, const int64_t *nmesh_host, cons
 int nbk_bispec_fill_poles(const void *cplx, int dtype, const int64_t *nmesh_host, const double *box_host, int layout,
                           int64_t start, int64_t count, const double *k2edges_host, int nedges, int shell0, int nshell,
                           const double *los_host, const int *ells_host, int nell, void *out, int64_t out_stride, void *stream);
+int nbk_bispec_fill_cross(const void *cplx, const void *cplx2, int dtype, const int64_t *nmesh_host, const double *box_host,
+                          int layout, int64_t start, int64_t count, const double *k2edges_host, int nedges, int shell0,
+                          int nshell, double scale, void *out, int64_t out_stride, void *stream);
 int nbk_bispec_triple_sum(const void *fields, int dtype, int64_t field_stride, int nfield, int64_t ncell, const int *triples,
                           int64_t ntri, double *out, void *stream);
 

@@ -280,97 +280,9 @@ class FFTBispectrum(FFTBase):
         return self.bispec
 
     def _pass(self, c, kedges, triples, indicator, ells=()):
-        """sum_x f_a f_b f_c for every row of `triples`, over the fields f = (family, shell) with field id
-        family * nshell + shell: family 0 is I (c 1_S in the mesh precision) or, indicator=True, J (1_S in float64);
-        family q > 0 is W^ell = c L_ell(mu) 1_S in the mesh precision, ell = ells[q - 1].
-        Returns the (nrow,) float64 device sums of this rank's x slab and the number of c2r transforms run."""
-        pm = c.pm if not indicator else c.pm.reshape(dtype='f8')
-        nshell = len(kedges) - 1
-        nfield = nshell * (1 + len(ells))
-        ntri = len(triples)
-        dev = c.value.device
-        code = _CODE[pm.typestr]
-        tdt = torch.float64 if pm.typestr == 'f8' else torch.float32
-        cdt = torch.complex128 if pm.typestr == 'f8' else torch.complex64
-        ncell = int(numpy.prod(pm.real_shape))
-        cslab = int(numpy.prod(pm.complex_shape))
-        fill_n = min(_FILL_CHUNK, nfield)
-        # the fill scratch, the transform's work buffers and a margin stay free
-        reserve = (fill_n + 4) * cslab * torch.empty((), dtype=cdt).element_size() + (256 << 20)
-        cap = _resident_cap(nfield, ncell * torch.empty((), dtype=tdt).element_size(), reserve, pm.comm)
-        # row groups, each run with its fields resident: everything at once; or one family at a time (its rows need
-        # W of that family and I); or, per family, shell blocks of cap // 3 so that any three of them are resident
-        # together.  A row's family is that of its first field (b and c are I fields).
-        rfam = triples[:, 0] // nshell
-        if cap >= nfield:
-            bsz, rfam = nshell, numpy.zeros_like(rfam)
-        else:
-            bsz = nshell if cap >= 2 * nshell else cap // 3
-        key = numpy.column_stack([rfam, (triples % nshell) // bsz])   # (nrow, 4); shell blocks non-decreasing in b, c
-        order = (numpy.lexsort((key[:, 3], key[:, 2], key[:, 1], key[:, 0])) if ntri
-                 else numpy.zeros(0, dtype='i8'))
-        store = torch.empty((min(cap, nfield), ncell), dtype=tdt, device=dev)
-        scratch = torch.empty((fill_n,) + tuple(pm.complex_shape), dtype=cdt, device=dev)
-        out = torch.zeros(ntri, dtype=torch.float64, device=dev)
-        tr, start, count = c._slab()
-        k2edges = _lib.darr((numpy.asarray(kedges) ** 2).astype('f8'))
-        los = _lib.darr([float(v) for v in self.attrs['los']])
-        slot_of = {}                                          # resident field -> row of `store`
-        transforms = 0
-        g0 = 0
-        while g0 < ntri:
-            g1 = g0
-            while g1 < ntri and (key[order[g1]] == key[order[g0]]).all():
-                g1 += 1
-            rows = order[g0:g1]
-            need = sorted(set(triples[rows].reshape(-1).tolist()))
-            for s in [s for s in slot_of if s not in need]:
-                del slot_of[s]
-            free = sorted(set(range(store.shape[0])) - set(slot_of.values()))
-            missing = [s for s in need if s not in slot_of]
-            for s in missing:
-                slot_of[s] = free.pop(0)
-            # contiguous runs of missing family-0 shells, each filled in chunks of at most fill_n shells by one read of c
-            runs = []
-            for s in missing:
-                if s >= nshell:
-                    break
-                if runs and runs[-1][-1] == s - 1 and len(runs[-1]) < fill_n:
-                    runs[-1].append(s)
-                else:
-                    runs.append([s])
-            for run in runs:
-                with stage("bispec_fill"):
-                    check(lib().nbk_bispec_fill(_ptr(c.value), _CODE[c.pm.typestr] if not indicator else code, pm._nmesh_c,
-                                                pm._box_c, tr, start, count, k2edges, len(kedges), run[0], len(run),
-                                                1 if indicator else 0, _ptr(scratch), cslab, _stream()), "nbk_bispec_fill")
-                for q, s in enumerate(run):
-                    with stage("bispec_c2r"):
-                        ComplexField(pm, scratch[q]).c2r(out=RealField(pm, store[slot_of[s]].view(pm.real_shape)))
-                    transforms += 1
-            # the missing weighted fields: one read of c per chunk of families x contiguous shells
-            for fams, run in _pole_chunks([s for s in missing if s >= nshell], nshell, fill_n):
-                with stage("bispec_fill_poles"):
-                    check(lib().nbk_bispec_fill_poles(_ptr(c.value), code, pm._nmesh_c, pm._box_c, tr, start, count, k2edges,
-                                                      len(kedges), run[0], len(run), los,
-                                                      _lib.i32arr([ells[f - 1] for f in fams]), len(fams), _ptr(scratch),
-                                                      cslab, _stream()), "nbk_bispec_fill_poles")
-                for q, f in enumerate(fams):
-                    for p, s in enumerate(run):
-                        with stage("bispec_c2r"):
-                            ComplexField(pm, scratch[q * len(run) + p]).c2r(
-                                out=RealField(pm, store[slot_of[f * nshell + s]].view(pm.real_shape)))
-                        transforms += 1
-            slots = numpy.vectorize(slot_of.get, otypes=['i4'])(triples[rows]) if len(rows) else None
-            tri_dev = torch.from_numpy(numpy.ascontiguousarray(slots, dtype='i4')).to(dev)
-            part = torch.zeros(len(rows), dtype=torch.float64, device=dev)
-            with stage("bispec_triple_sum"):
-                check(lib().nbk_bispec_triple_sum(_ptr(store), code, ncell, store.shape[0], ncell, _ptr(tri_dev), len(rows),
-                                                  _ptr(part), _stream()), "nbk_bispec_triple_sum")
-            out[torch.from_numpy(rows).to(dev)] = part
-            g0 = g1
-        del store, scratch
-        return out, transforms
+        """sum_x f_a f_b f_c for every row of `triples` (shell_pass), the weighted families those of `ells` about
+        attrs['los']"""
+        return shell_pass(c, kedges, triples, indicator, ells, los=self.attrs['los'])
 
     def __getstate__(self):
         return dict(bispec=self.bispec.__getstate__(), power=self.power.__getstate__(),
@@ -384,6 +296,135 @@ class FFTBispectrum(FFTBase):
         self.poles = None
         if state.get('poles') is not None:                   # results saved before multipoles have no 'poles'
             self.poles = BinnedStatistic.from_state(state['poles'])
+
+
+def shell_pass(c, kedges, triples, indicator, ells=(), los=None, sources=()):
+    """sum_x f_a f_b f_c for every row of `triples`, over the fields f = (family, shell) with field id
+    family * nshell + shell: family 0 is I (c 1_S in the mesh precision) or, indicator=True, J (1_S in float64);
+    family q > 0 is W^ell = c L_ell(mu) 1_S in the mesh precision, ell = ells[q - 1], mu about the unit 3-vector `los`.
+    With `sources` instead of `ells`, family q > 0 is filled from its own compressed field(s) on c's mesh and layout:
+    sources[q - 1] = ('field', G) gives G 1_S in the mesh precision (indicator=False), ('cross', G, D, scale) the
+    float64 scale G conj(D) 1_S (indicator=True: it shares the float64 store of J).
+    Returns the (nrow,) float64 device sums of this rank's x slab and the number of c2r transforms run."""
+    assert not (len(ells) and len(sources))
+    pm = c.pm if not indicator else c.pm.reshape(dtype='f8')
+    nshell = len(kedges) - 1
+    nfam = len(sources) if len(sources) else len(ells)
+    nfield = nshell * (1 + nfam)
+    ntri = len(triples)
+    dev = c.value.device
+    code = _CODE[pm.typestr]
+    tdt = torch.float64 if pm.typestr == 'f8' else torch.float32
+    cdt = torch.complex128 if pm.typestr == 'f8' else torch.complex64
+    ncell = int(numpy.prod(pm.real_shape))
+    cslab = int(numpy.prod(pm.complex_shape))
+    fill_n = min(_FILL_CHUNK, nfield)
+    # the fill scratch, the transform's work buffers and a margin stay free
+    reserve = (fill_n + 4) * cslab * torch.empty((), dtype=cdt).element_size() + (256 << 20)
+    cap = _resident_cap(nfield, ncell * torch.empty((), dtype=tdt).element_size(), reserve, pm.comm)
+    # row groups, each run with its fields resident: everything at once; or one family at a time (its rows need
+    # W of that family and I); or, per family, shell blocks of cap // 3 so that any three of them are resident
+    # together.  A row's family is that of its first field (b and c are I fields).
+    rfam = triples[:, 0] // nshell
+    if cap >= nfield:
+        bsz, rfam = nshell, numpy.zeros_like(rfam)
+    else:
+        bsz = nshell if cap >= 2 * nshell else cap // 3
+    key = numpy.column_stack([rfam, (triples % nshell) // bsz])   # (nrow, 4); shell blocks non-decreasing in b, c
+    order = (numpy.lexsort((key[:, 3], key[:, 2], key[:, 1], key[:, 0])) if ntri
+             else numpy.zeros(0, dtype='i8'))
+    store = torch.empty((min(cap, nfield), ncell), dtype=tdt, device=dev)
+    scratch = torch.empty((fill_n,) + tuple(pm.complex_shape), dtype=cdt, device=dev)
+    out = torch.zeros(ntri, dtype=torch.float64, device=dev)
+    tr, start, count = c._slab()
+    k2edges = _lib.darr((numpy.asarray(kedges) ** 2).astype('f8'))
+    los = _lib.darr([float(v) for v in los]) if len(ells) else None
+    slot_of = {}                                          # resident field -> row of `store`
+    transforms = 0
+    g0 = 0
+    while g0 < ntri:
+        g1 = g0
+        while g1 < ntri and (key[order[g1]] == key[order[g0]]).all():
+            g1 += 1
+        rows = order[g0:g1]
+        need = sorted(set(triples[rows].reshape(-1).tolist()))
+        for s in [s for s in slot_of if s not in need]:
+            del slot_of[s]
+        free = sorted(set(range(store.shape[0])) - set(slot_of.values()))
+        missing = [s for s in need if s not in slot_of]
+        for s in missing:
+            slot_of[s] = free.pop(0)
+        # contiguous runs of missing family-0 shells, each filled in chunks of at most fill_n shells by one read of c
+        runs = []
+        for s in missing:
+            if s >= nshell:
+                break
+            if runs and runs[-1][-1] == s - 1 and len(runs[-1]) < fill_n:
+                runs[-1].append(s)
+            else:
+                runs.append([s])
+        for run in runs:
+            with stage("bispec_fill"):
+                check(lib().nbk_bispec_fill(_ptr(c.value), _CODE[c.pm.typestr] if not indicator else code, pm._nmesh_c,
+                                            pm._box_c, tr, start, count, k2edges, len(kedges), run[0], len(run),
+                                            1 if indicator else 0, _ptr(scratch), cslab, _stream()), "nbk_bispec_fill")
+            for q, s in enumerate(run):
+                with stage("bispec_c2r"):
+                    ComplexField(pm, scratch[q]).c2r(out=RealField(pm, store[slot_of[s]].view(pm.real_shape)))
+                transforms += 1
+        # families with their own sources: contiguous runs of missing shells, one read of the source per run
+        for f, src in enumerate(sources, 1):
+            fruns = []
+            for s in [s % nshell for s in missing if s // nshell == f]:
+                if fruns and fruns[-1][-1] == s - 1 and len(fruns[-1]) < fill_n:
+                    fruns[-1].append(s)
+                else:
+                    fruns.append([s])
+            for run in fruns:
+                _fill_source(src, kedges, k2edges, run, tr, start, count, scratch, cslab)
+                for q, s in enumerate(run):
+                    with stage("bispec_c2r"):
+                        ComplexField(pm, scratch[q]).c2r(out=RealField(pm, store[slot_of[f * nshell + s]].view(pm.real_shape)))
+                    transforms += 1
+        # the missing weighted fields: one read of c per chunk of families x contiguous shells
+        for fams, run in _pole_chunks([s for s in missing if s >= nshell] if len(ells) else [], nshell, fill_n):
+            with stage("bispec_fill_poles"):
+                check(lib().nbk_bispec_fill_poles(_ptr(c.value), code, pm._nmesh_c, pm._box_c, tr, start, count, k2edges,
+                                                  len(kedges), run[0], len(run), los,
+                                                  _lib.i32arr([ells[f - 1] for f in fams]), len(fams), _ptr(scratch),
+                                                  cslab, _stream()), "nbk_bispec_fill_poles")
+            for q, f in enumerate(fams):
+                for p, s in enumerate(run):
+                    with stage("bispec_c2r"):
+                        ComplexField(pm, scratch[q * len(run) + p]).c2r(
+                            out=RealField(pm, store[slot_of[f * nshell + s]].view(pm.real_shape)))
+                    transforms += 1
+        slots = numpy.vectorize(slot_of.get, otypes=['i4'])(triples[rows]) if len(rows) else None
+        tri_dev = torch.from_numpy(numpy.ascontiguousarray(slots, dtype='i4')).to(dev)
+        part = torch.zeros(len(rows), dtype=torch.float64, device=dev)
+        with stage("bispec_triple_sum"):
+            check(lib().nbk_bispec_triple_sum(_ptr(store), code, ncell, store.shape[0], ncell, _ptr(tri_dev), len(rows),
+                                              _ptr(part), _stream()), "nbk_bispec_triple_sum")
+        out[torch.from_numpy(rows).to(dev)] = part
+        g0 = g1
+    del store, scratch
+    return out, transforms
+
+
+def _fill_source(src, kedges, k2edges, run, tr, start, count, scratch, cslab):
+    """one read of a shell_pass source field writes its shells `run` (contiguous) into the scratch slabs"""
+    G = src[1]
+    pm = G.pm
+    if src[0] == 'field':
+        with stage("bispec_fill"):
+            check(lib().nbk_bispec_fill(_ptr(G.value), _CODE[pm.typestr], pm._nmesh_c, pm._box_c, tr, start, count, k2edges,
+                                        len(kedges), run[0], len(run), 0, _ptr(scratch), cslab, _stream()), "nbk_bispec_fill")
+    else:
+        D, scale = src[2], float(src[3])
+        with stage("bispec_fill_cross"):
+            check(lib().nbk_bispec_fill_cross(_ptr(G.value), _ptr(D.value), _CODE[pm.typestr], pm._nmesh_c, pm._box_c, tr,
+                                              start, count, k2edges, len(kedges), run[0], len(run), scale, _ptr(scratch),
+                                              cslab, _stream()), "nbk_bispec_fill_cross")
 
 
 def _pole_chunks(fields, nshell, fill_n):

@@ -39,13 +39,35 @@ class FKPCatalogMesh(MultipleSpeciesCatalogMesh):
         self.nbar = nbar
 
     def __getitem__(self, key):
+        return self._species_mesh(key)
+
+    def _species_mesh(self, key, power=1):
+        """the species' CatalogMesh, each object of mass u^power (u = w_c w_fkp Value)"""
         assert key in self.source.species, "the species is not defined in the source"
         cat = self.source[key]
         assert cat.comm is self.comm
+        weight, value = self.TotalWeight(key), cat[self.value]
+        if power != 1:
+            weight, value = weight ** power, value ** power
         return CatalogMesh(cat, BoxSize=self.attrs['BoxSize'], Nmesh=self.attrs['Nmesh'], dtype=self.dtype,
-                           Weight=self.TotalWeight(key), Value=cat[self.value], Selection=cat[self.selection],
+                           Weight=weight, Value=value, Selection=cat[self.selection],
                            Position=self.RecenteredPosition(key), interlaced=self.interlaced,
                            compensated=self.compensated, resampler=self.resampler)
+
+    def to_shot_field(self):
+        """N = (sum_d u^2 W(x - x_d) + alpha^2 sum_r u^2 W(x - x_r)) / V_cell, painted as to_real_field paints F (same
+        window and interlacing) with mass u^2 and +alpha^2 in place of -alpha: the coincident-object field of the
+        bispectrum shot noise (ConvolvedFFTBispectrum)"""
+        wd, wr = self.weighted_total('data'), self.weighted_total('randoms')
+        alpha = wd / wr if wr != 0 else numpy.inf
+        real = self._species_mesh('data', 2).to_real_field(normalize=False)
+        if self.source['randoms'].csize > 0:
+            real2 = self._species_mesh('randoms', 2).to_real_field(normalize=False)
+            real.axpy(real2, alpha ** 2)
+            del real2
+        real /= (self.pm.BoxSize / self.pm.Nmesh).prod()
+        real.attrs = {'alpha': alpha}
+        return real
 
     def recenter_box(self, BoxSize, BoxCenter):
         """positions are re-centred to [-L/2, L/2] when painted (periodic wrap puts negatives in the upper half)"""

@@ -234,9 +234,6 @@ class ConvolvedFFTPower(object):
                 self.logger.info("normalization of power spectrum is neglected, as no random is provided.")
 
         comp = (compensation['first'], compensation['second'])
-        code = _CODE[pm.typestr]
-        tr, cstart, ccount = c1._slab()
-        off_c = _lib.darr(offset)
         proj = None
         start = time.time()
         # complex ('c16' / 'c8') meshes: the reference sums over ALL modes of a full mesh.  The field is real in
@@ -250,24 +247,10 @@ class ConvolvedFFTPower(object):
             work_r = RealField(pm)
             work_c = ComplexField(pm)
         for ell in poles[1:]:
-            Aell[...] = 0.
-            if full_mesh:
-                Bell[...] = 0.
             substart = time.time()
-            for m in range(-ell, ell + 1):
-                # F(x) Y_lm(xhat) -> FFT -> accumulate Y_lm(khat) * FFT
-                check(lib().nbk_ylm_mul_real(_ptr(rfield2.value), _ptr(work_r.value), code, ell, m, pm._nmesh_c,
-                                             pm._box_c, off_c, pm.x_start, pm.x_n, _stream()), "nbk_ylm_mul_real")
-                work_r.r2c(out=work_c)
-                if full_mesh:
-                    check(lib().nbk_ylm_mul_complex_acc2(_ptr(Aell.value), _ptr(Bell.value), _ptr(work_c.value), code, ell, m,
-                                                         pm._nmesh_c, pm._box_c, tr, cstart, ccount, _stream()),
-                          "nbk_ylm_mul_complex_acc2")
-                else:
-                    check(lib().nbk_ylm_mul_complex_acc(_ptr(Aell.value), _ptr(work_c.value), code, ell, m, pm._nmesh_c,
-                                                        pm._box_c, tr, cstart, ccount, _stream()), "nbk_ylm_mul_complex_acc")
-                if rank == 0:
-                    self.logger.debug("done term for Y(l=%d, m=%d) in %s" % (ell, m, timer(substart, time.time())))
+            ylm_multipole(rfield2, ell, offset, Aell, work_r, work_c, Bell)
+            if rank == 0:
+                self.logger.debug("done Y(l=%d, m) terms in %s" % (ell, timer(substart, time.time())))
             if rank == 0:
                 self.logger.info('ell = %d done; %s r2c completed' % (ell, 2 * ell + 1))
             # P_l = < norm * (V c1 / comp1) * conj(4 pi V Aell / comp2) >
@@ -344,6 +327,33 @@ class ConvolvedFFTPower(object):
 
 
 FKPPower = ConvolvedFFTPower
+
+
+def ylm_multipole(rfield, ell, offset, Aell, work_r, work_c, Bell=None):
+    """Aell = sum_m Y_lm(khat) r2c[F Y_lm(xhat)] over m = -ell .. ell (2 ell + 1 r2c), the field F = `rfield` of this
+    rank's x slab and xhat the unit vector of the cell coordinates + `offset` (BoxCenter + H / 2).  By the addition
+    theorem 4 pi Aell = (2 ell + 1) r2c[F L_ell(khat.xhat)].  `work_r` / `work_c` are scratch fields of rfield's mesh;
+    with `Bell` (full complex meshes) the mirror half is accumulated there as nbk_power_bin2 takes it."""
+    pm = rfield.pm
+    code = _CODE[pm.typestr]
+    tr, cstart, ccount = Aell._slab()
+    off_c = _lib.darr(offset)
+    Aell[...] = 0.
+    if Bell is not None:
+        Bell[...] = 0.
+    for m in range(-ell, ell + 1):
+        # F(x) Y_lm(xhat) -> FFT -> accumulate Y_lm(khat) * FFT
+        check(lib().nbk_ylm_mul_real(_ptr(rfield.value), _ptr(work_r.value), code, ell, m, pm._nmesh_c,
+                                     pm._box_c, off_c, pm.x_start, pm.x_n, _stream()), "nbk_ylm_mul_real")
+        work_r.r2c(out=work_c)
+        if Bell is not None:
+            check(lib().nbk_ylm_mul_complex_acc2(_ptr(Aell.value), _ptr(Bell.value), _ptr(work_c.value), code, ell, m,
+                                                 pm._nmesh_c, pm._box_c, tr, cstart, ccount, _stream()),
+                  "nbk_ylm_mul_complex_acc2")
+        else:
+            check(lib().nbk_ylm_mul_complex_acc(_ptr(Aell.value), _ptr(work_c.value), code, ell, m, pm._nmesh_c,
+                                                pm._box_c, tr, cstart, ccount, _stream()), "nbk_ylm_mul_complex_acc")
+    return Aell
 
 
 def _cast_mesh(mesh, Nmesh):

@@ -3,6 +3,8 @@
 //                            range of k shells (the inputs of the shell c2r transforms)
 //   nbk_bispec_fill_poles -- the same read writes c * L_ell(mu) * 1_S for a range of shells and several even ell (the
 //                            inputs of the multipole fields W^ell; mu = k.los / |k| in nbk_power_bin's float32 arithmetic)
+//   nbk_bispec_fill_cross -- one read of two compressed slabs writes scale * c * conj(d) * 1_S in float64 for a range of
+//                            shells (the shot-noise fields H of ConvolvedFFTBispectrum)
 //   nbk_bispec_triple_sum -- sum_x f_i f_j f_l over resident real x-slab fields for a device list of slot triples
 //
 // Built with --fmad=false: the shell of a mode is decided by the float32 coordinate arithmetic of nbk_power_bin
@@ -136,6 +138,44 @@ k_bispec_fill_poles(const typename Cplx<T>::type *__restrict__ c, FillParams P, 
     }
 }
 
+// One thread per mode of the slab (grid-stride), k_bispec_fill's shell rule in its own copy (so that the generated
+// code of k_bispec_fill and k_bispec_fill_poles stays as it was).  Output shell s starts s ostride complex float64
+// elements into `out` and holds scale * c * conj(d) at the modes of its shell, 0 elsewhere: the product of the two
+// mesh-precision values formed in float64.  For the spectra of two real fields the product is Hermitian.
+template <typename T>
+__global__ void __launch_bounds__(BS_THREADS)
+k_bispec_fill_cross(const typename Cplx<T>::type *__restrict__ c, const typename Cplx<T>::type *__restrict__ d, FillParams P,
+                    double scale, double2 *__restrict__ out) {
+    typedef typename Cplx<T>::type V2;
+    const SlabGeom &g = P.g;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < P.nelem; e += (int64_t)gridDim.x * blockDim.x) {
+        const int kz = (int)(e % g.Nzc);
+        const int64_t row = e / g.Nzc;
+        const int i1 = (int)(row % g.D1), i0 = (int)(row / g.D1);
+        int jx, jy, jz;
+        slab_freqs(g, i0, i1, kz, jx, jy, jz);
+        // (0 + kx^2) + ky^2, then + kz^2, in float32 as nbk_power_bin forms it
+        const float kx = (float)jx * P.kf32[0], ky = (float)jy * P.kf32[1], kzv = (float)jz * P.kf32[2];
+        const float kp2 = kx * kx + ky * ky;
+        const float k2 = kp2 + kzv * kzv;
+        const int b = nbk_k2_bin(P.k2e, P.nedge, (double)k2, (double)sqrtf(k2), P.kmin, P.inv_dk, P.uniform);
+        int local = b - 1 - P.shell0;
+        if (b < 1 || b >= P.nedge || (jx == 0 && jy == 0 && jz == 0)) local = -1;
+        double2 w = make_double2(0.0, 0.0);
+        if (local >= 0 && local < P.nshell) {
+            const V2 u = c[e], v = d[e];
+            const double ur = (double)u.x, ui = (double)u.y, vr = (double)v.x, vi = (double)v.y;
+            // (ur + i ui)(vr - i vi), every product rounded on its own (the file is built without FMA contraction)
+            const double re = ur * vr + ui * vi;
+            const double im = ui * vr - ur * vi;
+            w = make_double2(re * scale, im * scale);
+        }
+        const double2 z = make_double2(0.0, 0.0);
+        double2 *o = out + e;
+        for (int s = 0; s < P.nshell; s++) o[s * P.ostride] = (s == local) ? w : z;
+    }
+}
+
 // Block (x, y): the cell tiles x, x + gridDim.x, ... and the triples [y BS_TPT BS_THREADS, (y + 1) BS_TPT BS_THREADS).
 // A tile of BS_TILE cells of every resident field is staged in shared memory (rows padded by one element against bank
 // conflicts); each thread then adds f_i f_j f_l over the tile for its BS_TPT triples, the product formed and the sum
@@ -261,6 +301,29 @@ extern "C" int nbk_bispec_fill_poles(const void *cplx, int dtype, const int64_t 
         k_bispec_fill_poles<float><<<grid, BS_THREADS, 0, s>>>((const float2 *)cplx, P, L, out);
     } else {
         k_bispec_fill_poles<double><<<grid, BS_THREADS, 0, s>>>((const double2 *)cplx, P, L, out);
+    }
+    NBK_LAUNCHED();
+    return NBK_OK;
+}
+
+extern "C" int nbk_bispec_fill_cross(const void *cplx, const void *cplx2, int dtype, const int64_t *nmesh_host,
+                                     const double *box_host, int layout, int64_t start, int64_t count,
+                                     const double *k2edges_host, int nedges, int shell0, int nshell, double scale, void *out,
+                                     int64_t out_stride, void *stream) {
+    FillParams P;
+    int rc = make_fill(dtype, nmesh_host, box_host, layout, start, count, k2edges_host, nedges, shell0, nshell, nshell,
+                       out_stride, P);
+    if (rc) return rc;
+    NBK_CHECK_ARG(out != nullptr && cplx != nullptr && cplx2 != nullptr, "bispec_fill_cross: null field");
+    if (P.nelem == 0 || nshell == 0) return NBK_OK;
+    cudaStream_t s = (cudaStream_t)stream;
+    const int grid = nbk_grid_for(P.nelem, BS_THREADS, 8);
+    if (dtype == NBK_F4) {
+        k_bispec_fill_cross<float><<<grid, BS_THREADS, 0, s>>>((const float2 *)cplx, (const float2 *)cplx2, P, scale,
+                                                               (double2 *)out);
+    } else {
+        k_bispec_fill_cross<double><<<grid, BS_THREADS, 0, s>>>((const double2 *)cplx, (const double2 *)cplx2, P, scale,
+                                                                (double2 *)out);
     }
     NBK_LAUNCHED();
     return NBK_OK;
