@@ -261,7 +261,8 @@ int nbk_power_bin2(const void *c1, const void *c2, const void *c2_mirror, int dt
 
 /* out = c1 * conj(c2) * scale with element 0 cleared when clear_first != 0 (the k = 0 mode on the rank that owns
  * it): FFTBase._compute_3d_power (algorithms/fftpower.py:115-128), materialised only where the 3-D power itself
- * is needed (FFTCorr, algorithms/fftcorr.py:148-150).  c2 == NULL -> auto power.  out may alias c1. */
+ * is needed (FFTCorr, algorithms/fftcorr.py:148-150; FFT3PCF's kernel products).  c2 == NULL -> auto power.  out may
+ * alias c1 or c2: every element's inputs are read before that element is written. */
 int nbk_cross_power(const void *c1, const void *c2, void *out, int dtype, int64_t n_complex, double scale,
                     int clear_first, void *stream);
 
@@ -465,6 +466,24 @@ int nbk_bispec_fill_cross(const void *cplx, const void *cplx2, int dtype, const 
                           int nshell, double scale, void *out, int64_t out_stride, void *stream);
 int nbk_bispec_triple_sum(const void *fields, int dtype, int64_t field_stride, int nfield, int64_t ncell, const int *triples,
                           int64_t ntri, double *out, void *stream);
+
+/* FFT three-point correlation function of a periodic box (algorithms/fft3pcf.py: FFT3PCF; DESIGN.md 4.16).
+ *   kernel_fill : on the local x slab [x_start, x_start + x_n) of a real mesh (layout [x_n][Ny][Nz], dtype), writes for
+ *                 the real orthonormal harmonics m = m0 .. m0 + nm - 1 of multipole ell (m > 0: sqrt(2) Re Y_lm, m < 0:
+ *                 sqrt(2) Im Y_l|m|) the fields out[q][slab] = Y_l(m0+q)(s / r) at the cells whose grid separation s =
+ *                 (n_x H_x, n_y H_y, n_z H_z), n_i in (-N_i/2, N_i/2], H_i = box_i / N_i, has edges[bin] < r <= edges[bin
+ *                 + 1] and r > 0, r = sqrt((sx^2 + sy^2) + sz^2) in float64; 0 at every other cell; out_stride elements
+ *                 apart.  coef_host is SimulationBox3PCF's coefficient_table(L) ((L + 1)(L + 2) / 2 rows of L + 1,
+ *                 ell <= L <= 10); Y_lm is evaluated in float64 and rounded once to dtype.
+ *   gram        : w, A and B are real fields of ncell values (dtype); A holds na fields a_stride apart, B nb fields
+ *                 b_stride apart (1 .. 32 each).  Accumulates (device, zero first) out[i][j] +=
+ *                 sum_x w a_i b_j, row-major na x nb, products and sums in float64.  When B is A (same pointer, count
+ *                 and stride) only the entries i <= j are added. */
+int nbk_fft3pcf_kernel_fill(void *out, int dtype, const int64_t *nmesh_host, const double *box_host, int64_t x_start,
+                            int64_t x_n, const double *edges_host, int nedges, int bin, int ell, int m0, int nm,
+                            const double *coef_host, int L, int64_t out_stride, void *stream);
+int nbk_fft3pcf_gram(const void *w, const void *A, int64_t a_stride, int na, const void *B, int64_t b_stride, int nb,
+                     int dtype, int64_t ncell, double *out, void *stream);
 
 /* Cylindrical groups (algorithms/cgm.py: CylindricalGroups; DESIGN.md 4.9).  Rows key-sorted on a grid of ncell_host[d]
  * cells of side box[d] / ncell[d] as for nbk_paircount: spos double [n][3] (periodic: already wrapped), sprio[n] the

@@ -30,6 +30,7 @@ SOURCES = [
     ("zhist.cu", ["--fmad=false"]),
     ("hod.cu", ["--fmad=false"]),
     ("bispectrum.cu", ["--fmad=false"]),
+    ("fft3pcf.cu", ["--fmad=false"]),
 ]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ARCH + [ "-O3", "-lineinfo", "-std=c++17",

@@ -12,9 +12,10 @@ from .threeptcf import SimulationBox3PCF, SurveyData3PCF
 from .surveypaircount import SurveyDataPairCount, SurveyData2PCF
 from .convpower import ConvolvedFFTPower, FKPCatalog, FKPWeightFromNbar, FKPCatalogMesh
 from .convbispectrum import ConvolvedFFTBispectrum
+from .fft3pcf import FFT3PCF
 
 FKPPower = ConvolvedFFTPower
 
 __all__ = ['FOF', 'CylindricalGroups', 'KDDensity', 'FiberCollisions', 'RedshiftHistogram', 'SimulationBoxPairCount', 'SimulationBox2PCF', 'SimulationBox3PCF', 'SurveyDataPairCount',
-           'SurveyData2PCF', 'SurveyData3PCF', 'FFTCorr', 'FFTRecon', 'FFTPower', 'FFTBispectrum', 'ProjectedFFTPower', 'FFTBase', 'project_to_basis', 'ConvolvedFFTPower', 'ConvolvedFFTBispectrum', 'FKPPower', 'FKPCatalog',
+           'SurveyData2PCF', 'SurveyData3PCF', 'FFT3PCF', 'FFTCorr', 'FFTRecon', 'FFTPower', 'FFTBispectrum', 'ProjectedFFTPower', 'FFTBase', 'project_to_basis', 'ConvolvedFFTPower', 'ConvolvedFFTBispectrum', 'FKPPower', 'FKPCatalog',
            'FKPWeightFromNbar', 'FKPCatalogMesh']
