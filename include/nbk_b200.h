@@ -478,12 +478,18 @@ int nbk_bispec_triple_sum(const void *fields, int dtype, int64_t field_stride, i
  *   gram        : w, A and B are real fields of ncell values (dtype); A holds na fields a_stride apart, B nb fields
  *                 b_stride apart (1 .. 32 each).  Accumulates (device, zero first) out[i][j] +=
  *                 sum_x w a_i b_j, row-major na x nb, products and sums in float64.  When B is A (same pointer, count
- *                 and stride) only the entries i <= j are added. */
+ *                 and stride) only the entries i <= j are added.
+ *   gram_tiles  : gram over the cells of the tiles tiles[0 .. ntiles) only (device int64, each in [0, ceil(ncell / 64)),
+ *                 tile t = cells 64 t .. 64 t + 63); w must be 0 on every cell of the tiles left out, so the sum is
+ *                 gram's up to summation order (algorithms/convfft3pcf.py: ConvolvedFFT3PCF; DESIGN.md 4.17). */
 int nbk_fft3pcf_kernel_fill(void *out, int dtype, const int64_t *nmesh_host, const double *box_host, int64_t x_start,
                             int64_t x_n, const double *edges_host, int nedges, int bin, int ell, int m0, int nm,
                             const double *coef_host, int L, int64_t out_stride, void *stream);
 int nbk_fft3pcf_gram(const void *w, const void *A, int64_t a_stride, int na, const void *B, int64_t b_stride, int nb,
                      int dtype, int64_t ncell, double *out, void *stream);
+int nbk_fft3pcf_gram_tiles(const void *w, const void *A, int64_t a_stride, int na, const void *B, int64_t b_stride,
+                           int nb, int dtype, int64_t ncell, const int64_t *tiles, int64_t ntiles, double *out,
+                           void *stream);
 
 /* Cylindrical groups (algorithms/cgm.py: CylindricalGroups; DESIGN.md 4.9).  Rows key-sorted on a grid of ncell_host[d]
  * cells of side box[d] / ncell[d] as for nbk_paircount: spos double [n][3] (periodic: already wrapped), sprio[n] the

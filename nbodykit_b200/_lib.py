@@ -107,6 +107,7 @@ SIGNATURES = {
     "nbk_bispec_triple_sum": ([_vp, _i, _i64, _i, _i64, _vp, _i64, _vp, _vp], _i),
     "nbk_fft3pcf_kernel_fill": ([_vp, _i, _pi64, _pd, _i64, _i64, _pd, _i, _i, _i, _i, _i, _pd, _i, _i64, _vp], _i),
     "nbk_fft3pcf_gram": ([_vp, _vp, _i64, _i, _vp, _i64, _i, _i, _i64, _vp, _vp], _i),
+    "nbk_fft3pcf_gram_tiles": ([_vp, _vp, _i64, _i, _vp, _i64, _i, _i, _i64, _vp, _i64, _vp, _vp], _i),
     "nbk_cgm_chunk_rows": ([], _i64),
     "nbk_cgm_count": ([_vp, _vp, _vp, _i64, _i64, _vp, _vp, _i64, _vp, _vp, _i64, _i, _pd, _pi64, _pd, _pd, _d, _d, _vp, _vp,
                        _vp], _i),

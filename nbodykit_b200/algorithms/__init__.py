@@ -13,9 +13,10 @@ from .surveypaircount import SurveyDataPairCount, SurveyData2PCF
 from .convpower import ConvolvedFFTPower, FKPCatalog, FKPWeightFromNbar, FKPCatalogMesh
 from .convbispectrum import ConvolvedFFTBispectrum
 from .fft3pcf import FFT3PCF
+from .convfft3pcf import ConvolvedFFT3PCF
 
 FKPPower = ConvolvedFFTPower
 
 __all__ = ['FOF', 'CylindricalGroups', 'KDDensity', 'FiberCollisions', 'RedshiftHistogram', 'SimulationBoxPairCount', 'SimulationBox2PCF', 'SimulationBox3PCF', 'SurveyDataPairCount',
-           'SurveyData2PCF', 'SurveyData3PCF', 'FFT3PCF', 'FFTCorr', 'FFTRecon', 'FFTPower', 'FFTBispectrum', 'ProjectedFFTPower', 'FFTBase', 'project_to_basis', 'ConvolvedFFTPower', 'ConvolvedFFTBispectrum', 'FKPPower', 'FKPCatalog',
+           'SurveyData2PCF', 'SurveyData3PCF', 'FFT3PCF', 'FFTCorr', 'FFTRecon', 'FFTPower', 'FFTBispectrum', 'ProjectedFFTPower', 'FFTBase', 'project_to_basis', 'ConvolvedFFTPower', 'ConvolvedFFTBispectrum', 'ConvolvedFFT3PCF', 'FKPPower', 'FKPCatalog',
            'FKPWeightFromNbar', 'FKPCatalogMesh']

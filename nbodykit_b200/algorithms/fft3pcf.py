@@ -25,10 +25,16 @@ from .fftpower import FFTBase
 from .threeptcf import _check_edges, _check_poles, coefficient_table
 
 
-def transform_count(blocks, poles):
-    """the r2c and c2r transforms of one call on the bin blocks `blocks` (bin_blocks): 1 for delta, then per (l, m)
-    two per kernel field built -- block p is built once as the first of its pairs and once for each earlier block"""
-    return 1 + 2 * sum(2 * ell + 1 for ell in poles) * sum(len(b) * (1 + p) for p, b in enumerate(blocks))
+# cells per tile of the Gram (F3_TILE of csrc/fft3pcf.cu): the unit of the tile lists of nbk_fft3pcf_gram_tiles
+GRAM_TILE = 64
+
+
+def transform_count(blocks, poles, sources=1):
+    """the r2c and c2r transforms of one call on the bin blocks `blocks` (bin_blocks) with `sources` weighted fields
+    (bin_pass): one r2c per field, then per (l, m) one r2c per kernel field built and one c2r per field -- block p is
+    built once as the first of its pairs and once for each earlier block"""
+    return sources + (1 + sources) * sum(2 * ell + 1 for ell in poles) * sum(len(b) * (1 + p)
+                                                                           for p, b in enumerate(blocks))
 
 
 def bin_blocks(nbins, cap):
@@ -61,6 +67,121 @@ def separation_counts(Nmesh, BoxSize, edges):
         ok = (r > 0) & (b >= 0) & (b < nb)
         counts += numpy.bincount(b[ok], minlength=nb).astype('u8')
     return counts
+
+
+def tile_list(w):
+    """the indices (device int64) of the GRAM_TILE-cell tiles of the local field `w` (RealField) that hold a nonzero
+    cell: the tiles nbk_fft3pcf_gram_tiles visits.  Its sum over them is the dense Gram's, as w = 0 on the others."""
+    v = w.value.reshape(-1)
+    pad = (-v.numel()) % GRAM_TILE
+    if pad:
+        v = torch.cat([v, v.new_zeros(pad)])
+    return torch.nonzero((v.view(-1, GRAM_TILE) != 0).any(dim=1)).reshape(-1)
+
+
+def bin_pass(pm, sources, edges, poles):
+    """the Gram sums of FFT3PCF and ConvolvedFFT3PCF.  `sources` is a list of (w, what, tiles): a weight RealField w, the
+    spectrum what (ComplexField) of the field the bin kernels are applied to, and None (the dense Gram) or w's
+    tile_list (the listed Gram).  Per (l, m) and radial bin b the kernel field K = Y_lm 1_b is filled and transformed
+    once; per source, c2r(what conj(K^) N_cells) = sum_{s in b} Y_lm(s) f(x + s) goes to that source's resident store
+    (the last product is formed in K^'s own buffer, the others in scratch spectra), and one Gram per source and block
+    pair accumulates sum_x w a_i b_j.  Bins that do not fit run in blocks (bin_blocks; the stores of every source count
+    against free memory).  One all-reduce carries the packed float64 sums.
+
+    Returns the (len(sources), len(poles), nb, nb) host array (1 / 4 pi) sum_m sum_x w a_lm,b1 a_lm,b2 (all ranks) and
+    the number of transforms run (those of the spectra `what` not included)."""
+    e = numpy.asarray(edges, dtype='f8')
+    nb = len(e) - 1
+    nsrc = len(sources)
+    L = max(poles)
+    T = darr(numpy.ascontiguousarray(coefficient_table(L)).ravel())
+    code = _CODE[pm.typestr]
+    tdt = torch.float64 if pm.typestr == 'f8' else torch.float32
+    cdt = torch.complex128 if pm.typestr == 'f8' else torch.complex64
+    dev = sources[0][0].value.device
+    ncell = int(numpy.prod(pm.real_shape))
+    ncells = int(numpy.prod(pm.Nmesh))
+
+    # the kernel field, its spectrum, the scratch spectra, the transforms' work buffers and a margin stay free
+    cslab = int(numpy.prod(pm.complex_shape))
+    esz = torch.empty((), dtype=cdt).element_size()
+    fsz = ncell * torch.empty((), dtype=tdt).element_size()
+    reserve = (3 + nsrc) * cslab * esz + fsz + (256 << 20)
+    cap = _resident_cap(nb, nsrc * fsz, reserve, pm.comm)
+    blocks = bin_blocks(nb, cap)
+    bsz = len(blocks[0])
+    stores = [torch.empty((bsz if len(blocks) == 1 else 2 * bsz, ncell), dtype=tdt, device=dev) for _ in sources]
+    K = RealField(pm)
+    Khat = ComplexField(pm)
+    prods = [ComplexField(pm) for _ in sources[:-1]] + [Khat]
+    # one float64 accumulator per source, pole and block pair (p <= q), packed for the single all-reduce
+    pairs = [(p, q) for p in range(len(blocks)) for q in range(p, len(blocks))]
+    offs, o = {}, 0
+    for pq in pairs:
+        offs[pq] = o
+        o += len(blocks[pq[0]]) * len(blocks[pq[1]])
+    sums = torch.zeros((nsrc, len(poles), o), dtype=torch.float64, device=dev)
+    g = lib()
+    box = pm._box_c
+    edges_c = darr(e)
+    counted = [0]
+
+    def build(bins, row0, ell, m):
+        """a_lm,b of every source for the bins `bins` into store rows row0, row0 + 1, ..."""
+        for q, b in enumerate(bins):
+            with stage("fft3pcf_fill"):
+                check(g.nbk_fft3pcf_kernel_fill(_ptr(K.value), code, pm._nmesh_c, box, pm.x_start, pm.x_n, edges_c,
+                                                len(e), b, ell, m, 1, T, L, ncell, _stream()), "nbk_fft3pcf_kernel_fill")
+            with stage("fft3pcf_r2c"):
+                K.r2c(out=Khat)
+            with stage("fft3pcf_product"):
+                # what conj(K^) into the source's buffer, the last one into K^'s own (every element's inputs are read
+                # before it is written), times N_cells: c2r of the product is then sum_s K(s) f(x + s)
+                for (_, what, _), out in zip(sources, prods):
+                    check(g.nbk_cross_power(_ptr(what.value), _ptr(Khat.value), _ptr(out.value), code,
+                                            Khat.value.numel(), float(ncells), 0, _stream()), "nbk_cross_power")
+            with stage("fft3pcf_c2r"):
+                for out, store in zip(prods, stores):
+                    out.c2r(out=RealField(pm, store[row0 + q].view(pm.real_shape)))
+            counted[0] += 1 + nsrc
+
+    def gram(p, pa, pb):
+        """sum_x w a_i b_j of the resident blocks: pa from store row 0, pb (when another block) from row bsz"""
+        A, B = blocks[pa], blocks[pb]
+        rowb = 0 if pa == pb else bsz
+        with stage("fft3pcf_gram"):
+            for s, ((w, _, tiles), store) in enumerate(zip(sources, stores)):
+                out = sums[s, p, offs[(pa, pb)]:]
+                if tiles is None:
+                    check(g.nbk_fft3pcf_gram(_ptr(w.value), _ptr(store[0]), ncell, len(A), _ptr(store[rowb]), ncell,
+                                             len(B), code, ncell, _ptr(out), _stream()), "nbk_fft3pcf_gram")
+                else:
+                    check(g.nbk_fft3pcf_gram_tiles(_ptr(w.value), _ptr(store[0]), ncell, len(A), _ptr(store[rowb]),
+                                                   ncell, len(B), code, ncell, _ptr(tiles), tiles.numel(), _ptr(out),
+                                                   _stream()), "nbk_fft3pcf_gram_tiles")
+
+    for p, ell in enumerate(poles):
+        for m in range(-ell, ell + 1):
+            for pa in range(len(blocks)):
+                build(blocks[pa], 0, ell, m)
+                gram(p, pa, pa)
+                for pb in range(pa + 1, len(blocks)):
+                    build(blocks[pb], bsz, ell, m)
+                    gram(p, pa, pb)
+    del stores, K, Khat, prods
+    with stage("fft3pcf_allreduce"):
+        if pm.comm.size > 1:
+            pm.comm.allreduce_tensor(sums)
+    host = sums.cpu().numpy()
+    corr = numpy.zeros((nsrc, len(poles), nb, nb))
+    for (pa, pb) in pairs:
+        A, B = blocks[pa], blocks[pb]
+        part = host[:, :, offs[(pa, pb)]:offs[(pa, pb)] + len(A) * len(B)].reshape(nsrc, len(poles), len(A), len(B))
+        corr[:, :, A[0]:A[-1] + 1, B[0]:B[-1] + 1] = part
+    iu = numpy.triu_indices(nb, 1)
+    corr[:, :, iu[1], iu[0]] = corr[:, :, iu[0], iu[1]]             # the Gram adds i <= j of a block with itself
+    corr /= 4 * numpy.pi
+    return corr, counted[0]
 
 
 class FFT3PCF(FFTBase):
@@ -124,9 +245,6 @@ class FFT3PCF(FFTBase):
         attrs = self.attrs
         poles = attrs['poles']
         e = numpy.asarray(attrs['edges'], dtype='f8')
-        nb = len(e) - 1
-        L = max(poles)
-        T = darr(numpy.ascontiguousarray(coefficient_table(L)).ravel())
         with stage("fft3pcf_paint"):
             F = self.first.compute(mode='real', Nmesh=attrs['Nmesh'])
         attrs['N1'] = F.attrs.get('N', 0)
@@ -136,11 +254,6 @@ class FFT3PCF(FFTBase):
             # a complex-typed mesh stores its real field as a real array: the real-dtype mesh takes it as it is
             pm = pm.reshape(dtype=pm.typestr)
             F = RealField(pm, F.value)
-        code = _CODE[pm.typestr]
-        tdt = torch.float64 if pm.typestr == 'f8' else torch.float32
-        cdt = torch.complex128 if pm.typestr == 'f8' else torch.complex64
-        dev = F.value.device
-        ncell = int(numpy.prod(pm.real_shape))
         ncells = int(numpy.prod(pm.Nmesh))
         with stage("fft3pcf_mean"):
             mean = F.csum() / ncells                               # the one all-reduce of the mean
@@ -151,81 +264,11 @@ class FFT3PCF(FFTBase):
         del F
         with stage("fft3pcf_r2c"):
             dhat = delta.r2c()
-
-        # the kernel field, its spectrum, the transforms' work buffers and a margin stay free
-        cslab = int(numpy.prod(pm.complex_shape))
-        esz = torch.empty((), dtype=cdt).element_size()
-        reserve = 4 * cslab * esz + ncell * torch.empty((), dtype=tdt).element_size() + (256 << 20)
-        cap = _resident_cap(nb, ncell * torch.empty((), dtype=tdt).element_size(), reserve, pm.comm)
-        blocks = bin_blocks(nb, cap)
-        bsz = len(blocks[0])
-        store = torch.empty((bsz if len(blocks) == 1 else 2 * bsz, ncell), dtype=tdt, device=dev)
-        K = RealField(pm)
-        Khat = ComplexField(pm)
-        # one float64 accumulator per pole and block pair (p <= q), packed for the single all-reduce
-        pairs = [(p, q) for p in range(len(blocks)) for q in range(p, len(blocks))]
-        offs, o = {}, 0
-        for pq in pairs:
-            offs[pq] = o
-            o += len(blocks[pq[0]]) * len(blocks[pq[1]])
-        sums = torch.zeros((len(poles), o), dtype=torch.float64, device=dev)
-        g = lib()
-        box = pm._box_c
-        edges_c = darr(e)
-
-        counted = [1]                                              # the transform of delta
-
-        def build(bins, row0, ell, m):
-            """a_lm,b for the bins `bins` into store rows row0, row0 + 1, ..."""
-            for q, b in enumerate(bins):
-                with stage("fft3pcf_fill"):
-                    check(g.nbk_fft3pcf_kernel_fill(_ptr(K.value), code, pm._nmesh_c, box, pm.x_start, pm.x_n, edges_c,
-                                                    len(e), b, ell, m, 1, T, L, ncell, _stream()),
-                          "nbk_fft3pcf_kernel_fill")
-                with stage("fft3pcf_r2c"):
-                    K.r2c(out=Khat)
-                with stage("fft3pcf_product"):
-                    # conj(K^) delta^ into K^'s buffer (every element's inputs are read before it is written), times
-                    # N_cells: c2r of the product is then sum_s K(s) delta(x + s)
-                    check(g.nbk_cross_power(_ptr(dhat.value), _ptr(Khat.value), _ptr(Khat.value), code,
-                                            Khat.value.numel(), float(ncells), 0, _stream()), "nbk_cross_power")
-                with stage("fft3pcf_c2r"):
-                    Khat.c2r(out=RealField(pm, store[row0 + q].view(pm.real_shape)))
-                counted[0] += 2
-
-        def gram(p, pa, pb):
-            """sum_x delta a_i b_j of the resident blocks: pa from store row 0, pb (when another block) from row bsz"""
-            A, B = blocks[pa], blocks[pb]
-            out = sums[p, offs[(pa, pb)]:]
-            rowb = 0 if pa == pb else bsz
-            with stage("fft3pcf_gram"):
-                check(g.nbk_fft3pcf_gram(_ptr(delta.value), _ptr(store[0]), ncell, len(A), _ptr(store[rowb]), ncell,
-                                         len(B), code, ncell, _ptr(out), _stream()), "nbk_fft3pcf_gram")
-
-        for p, ell in enumerate(poles):
-            for m in range(-ell, ell + 1):
-                for pa in range(len(blocks)):
-                    build(blocks[pa], 0, ell, m)
-                    gram(p, pa, pa)
-                    for pb in range(pa + 1, len(blocks)):
-                        build(blocks[pb], bsz, ell, m)
-                        gram(p, pa, pb)
-        del store, K, Khat, dhat, delta
-        with stage("fft3pcf_allreduce"):
-            if pm.comm.size > 1:
-                pm.comm.allreduce_tensor(sums)
-        host = sums.cpu().numpy()
-        corr = numpy.zeros((len(poles), nb, nb))
-        for (pa, pb) in pairs:
-            A, B = blocks[pa], blocks[pb]
-            part = host[:, offs[(pa, pb)]:offs[(pa, pb)] + len(A) * len(B)].reshape(len(poles), len(A), len(B))
-            corr[:, A[0]:A[-1] + 1, B[0]:B[-1] + 1] = part
-        iu = numpy.triu_indices(nb, 1)
-        corr[:, iu[1], iu[0]] = corr[:, iu[0], iu[1]]               # the Gram adds i <= j of a block with itself
-        corr /= 4 * numpy.pi
+        corr, n = bin_pass(pm, [(delta, dhat, None)], e, poles)
+        del dhat, delta
         self.nsep = separation_counts(pm.Nmesh, pm.BoxSize, e)
-        attrs['transforms'] = counted[0]
-        self.poles = BinnedStatistic(['r1', 'r2'], [e, e], pole_table(corr, self.nsep, ncells, poles))
+        attrs['transforms'] = 1 + n
+        self.poles = BinnedStatistic(['r1', 'r2'], [e, e], pole_table(corr[0], self.nsep, ncells, poles))
         return self.poles
 
     def __getstate__(self):

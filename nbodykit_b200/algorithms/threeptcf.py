@@ -116,6 +116,64 @@ def _check_poles(poles):
     return p
 
 
+def threej_squared(l1, l2, l3):
+    """the squared Wigner 3j symbol (l1 l2 l3; 0 0 0)^2 in closed form, exact (Fraction): 0 unless J = l1 + l2 + l3 is
+    even and the triangle rule holds; else, with g = J / 2,
+    (J - 2 l1)! (J - 2 l2)! (J - 2 l3)! / (J + 1)! [g! / ((g - l1)! (g - l2)! (g - l3)!)]^2"""
+    J = l1 + l2 + l3
+    if J % 2 or l3 > l1 + l2 or l3 < abs(l1 - l2):
+        return Fraction(0)
+    g = J // 2
+    f = math.factorial
+    a = Fraction(f(J - 2 * l1) * f(J - 2 * l2) * f(J - 2 * l3), f(J + 1))
+    b = Fraction(f(g), f(g - l1) * f(g - l2) * f(g - l3))
+    return a * b * b
+
+
+def edge_correct(nnn, rrr, poles):
+    r"""The edge-corrected multipoles :math:`\zeta_\ell(r_1, r_2)` of the 3PCF of a survey (Slepian and Eisenstein, MNRAS
+    454, 4142 (2015), §4), on the host in float64.
+
+    ``nnn`` and ``rrr`` are (len(poles), nb, nb) arrays of the multipoles of the weighted triplet counts of the FKP field
+    N = D - alpha R and of the randoms alpha R, in the same normalisation (any common factor cancels).  ``poles`` must
+    hold every ell from 0 to max(poles), in any order: the coupling system below is only consistent on a contiguous set.
+    For every bin pair, with n_l = nnn_l / rrr_0 and f_l = rrr_l / rrr_0,
+
+    .. math::
+
+        M_{\ell\ell'} = (2\ell + 1) \sum_{\ell'' \in poles} \begin{pmatrix} \ell & \ell' & \ell'' \\ 0 & 0 & 0
+            \end{pmatrix}^2 f_{\ell''}, \qquad \zeta = M^{-1} n
+
+    (NaN where rrr_0 = 0).  When R has no multipoles above max(poles) this is exact; otherwise it truncates them.
+
+    :class:`ConvolvedFFT3PCF` calls it on its own sums.  For the pair walk, run :class:`SimulationBox3PCF` with
+    ``periodic=False`` (or :class:`SurveyData3PCF`) twice on the data and randoms together: once with weights w_d for the
+    data rows and -alpha w_r for the random rows (``nnn``), and once on the random rows alone with weights alpha w_r
+    (``rrr``); pass the ``corr_<l>`` columns of the two results, stacked in the order of ``poles``.
+
+    Returns the (len(poles), nb, nb) array zeta, in the order of ``poles``.
+    """
+    poles = [int(ell) for ell in poles]
+    if sorted(poles) != list(range(max(poles) + 1)):
+        raise ValueError("edge_correct: poles must hold every ell from 0 to max(poles) (got %s)" % poles)
+    nnn = numpy.asarray(nnn, dtype='f8')
+    rrr = numpy.asarray(rrr, dtype='f8')
+    if nnn.shape != rrr.shape or nnn.ndim != 3 or nnn.shape[0] != len(poles):
+        raise ValueError("edge_correct: nnn and rrr must both have shape (len(poles), nb, nb)")
+    # C[a, c, k] = (2 l_a + 1) (l_a l_c l_k; 0 0 0)^2 over the poles' order
+    C = numpy.array([[[(2 * la + 1) * float(threej_squared(la, lc, lk)) for lk in poles] for lc in poles]
+                     for la in poles])
+    r0 = rrr[poles.index(0)]
+    ok = r0 != 0
+    zeta = numpy.full(nnn.shape, numpy.nan)
+    if ok.any():
+        n = nnn[:, ok] / r0[ok]                                  # (npoles, npairs)
+        f = rrr[:, ok] / r0[ok]
+        M = numpy.einsum('ack,kq->qac', C, f)                    # (npairs, npoles, npoles)
+        zeta[:, ok] = numpy.linalg.solve(M, n.T[:, :, None])[:, :, 0].T
+    return zeta
+
+
 def count_triplets(pos1, w1, pos2, w2, edges, poles, periodic, box):
     """zeta_l(b1, b2) of the primaries pos1 against the secondaries pos2 on this device, per the contract of DESIGN.md
     4.7, without the factor 1 / (16 pi^2) and with only b1 <= b2 filled.  pos: (n, 3) float32 / float64 device

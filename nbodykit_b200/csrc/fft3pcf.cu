@@ -3,6 +3,8 @@
 //                              m on the local x slab of a real mesh (the inputs of the kernel r2c transforms)
 //   nbk_fft3pcf_gram        -- out[i][j] += sum_x w a_i b_j over two sets of resident real x-slab fields, register-blocked
 //                              over the outer product (i <= j only when the two sets are the same)
+//   nbk_fft3pcf_gram_tiles  -- the same over a list of 64-cell tiles, for weight fields that are zero outside them
+//                              (algorithms/convfft3pcf.py: ConvolvedFFT3PCF; DESIGN.md 4.17)
 //
 // Built with --fmad=false: r = sqrt((sx^2 + sy^2) + sz^2) decides the bin of a grid separation, so no contraction may
 // move a separation across an edge; the Y_lm polynomials and the Gram sums use explicit fma().
@@ -84,12 +86,14 @@ __global__ void __launch_bounds__(F3_THREADS) k_fft3pcf_fill(KernelParams P, T *
 // (i, j) block t % nblk and the cells t / nblk, t / nblk + ngroup, ... of each tile: per cell it forms w a_i once for
 // its F3_BLK rows of A and adds (w a_i) b_j into F3_BLK^2 float64 registers.  SYM: B is A and only blocks with bi <= bj
 // exist.  At the end the groups' partial blocks are summed in shared memory and each (i, j) gets one float64 atomic
-// per block (diagonal blocks of SYM only add i <= j).
-template <typename T, bool SYM>
+// per block (diagonal blocks of SYM only add i <= j).  LIST: the block walks entries blockIdx.x, blockIdx.x + gridDim.x,
+// ... of the tile list tiles[ntiles] instead of every tile (a tile left out must have w = 0 on all its cells).
+template <typename T, bool SYM, bool LIST>
 __global__ void __launch_bounds__(F3_THREADS) k_fft3pcf_gram(const T *__restrict__ w, const T *__restrict__ A,
                                                              int64_t astride, int na, const T *__restrict__ B,
                                                              int64_t bstride, int nb, int64_t ncell,
-                                                             double *__restrict__ out) {
+                                                             double *__restrict__ out, const int64_t *__restrict__ tiles,
+                                                             int64_t ntiles) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     double *s = reinterpret_cast<double *>(smem_raw);
     const int RA = (na + F3_BLK - 1) / F3_BLK * F3_BLK;
@@ -120,9 +124,9 @@ __global__ void __launch_bounds__(F3_THREADS) k_fft3pcf_gram(const T *__restrict
 #pragma unroll
         for (int j = 0; j < F3_BLK; j++) acc[i][j] = 0.0;
     const int nrow = RA + RB + 1;
-    const int64_t ntile = (ncell + F3_TILE - 1) / F3_TILE;
-    for (int64_t tile = blockIdx.x; tile < ntile; tile += gridDim.x) {
-        const int64_t c0 = tile * F3_TILE;
+    const int64_t nwalk = LIST ? ntiles : (ncell + F3_TILE - 1) / F3_TILE;
+    for (int64_t it = blockIdx.x; it < nwalk; it += gridDim.x) {
+        const int64_t c0 = (LIST ? tiles[it] : it) * F3_TILE;
         __syncthreads();
         for (int idx = threadIdx.x; idx < nrow * F3_TILE; idx += F3_THREADS) {
             const int r = idx / F3_TILE, cc = idx - r * F3_TILE;
@@ -246,9 +250,9 @@ extern "C" int nbk_fft3pcf_kernel_fill(void *out, int dtype, const int64_t *nmes
     return NBK_OK;
 }
 
-template <typename T, bool SYM>
+template <typename T, bool SYM, bool LIST>
 static int launch_gram(const void *w, const void *A, int64_t astride, int na, const void *B, int64_t bstride, int nb,
-                       int64_t ncell, double *out, cudaStream_t s) {
+                       int64_t ncell, const int64_t *tiles, int64_t ntiles, double *out, cudaStream_t s) {
     const int RA = (na + F3_BLK - 1) / F3_BLK * F3_BLK;
     const int RB = SYM ? 0 : (nb + F3_BLK - 1) / F3_BLK * F3_BLK;
     const int nbi = RA / F3_BLK, nbj = SYM ? nbi : RB / F3_BLK;
@@ -257,35 +261,52 @@ static int launch_gram(const void *w, const void *A, int64_t astride, int na, co
     size_t smem = (size_t)F3_TILE * (RA + RB + 1) * sizeof(double);
     const size_t red = (size_t)ngroup * nblk * F3_BLK * F3_BLK * sizeof(double);
     if (red > smem) smem = red;
-    NBK_CUDA(cudaFuncSetAttribute(k_fft3pcf_gram<T, SYM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    NBK_CUDA(cudaFuncSetAttribute(k_fft3pcf_gram<T, SYM, LIST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int occ = 0;
-    NBK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_fft3pcf_gram<T, SYM>, F3_THREADS, smem));
+    NBK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_fft3pcf_gram<T, SYM, LIST>, F3_THREADS, smem));
     if (occ < 1) occ = 1;
-    const int64_t ntile = (ncell + F3_TILE - 1) / F3_TILE;
+    const int64_t nwalk = LIST ? ntiles : (ncell + F3_TILE - 1) / F3_TILE;
     int64_t gx = (int64_t)NBK_SM_COUNT * occ;
-    if (gx > ntile) gx = ntile;
+    if (gx > nwalk) gx = nwalk;
     if (gx < 1) gx = 1;
-    k_fft3pcf_gram<T, SYM><<<(unsigned)gx, F3_THREADS, smem, s>>>((const T *)w, (const T *)A, astride, na, (const T *)B,
-                                                                  bstride, nb, ncell, out);
+    k_fft3pcf_gram<T, SYM, LIST><<<(unsigned)gx, F3_THREADS, smem, s>>>((const T *)w, (const T *)A, astride, na,
+                                                                        (const T *)B, bstride, nb, ncell, out, tiles,
+                                                                        ntiles);
     NBK_LAUNCHED();
     return NBK_OK;
 }
 
-extern "C" int nbk_fft3pcf_gram(const void *w, const void *A, int64_t a_stride, int na, const void *B, int64_t b_stride,
-                                int nb, int dtype, int64_t ncell, double *out, void *stream) {
-    NBK_CHECK_ARG(dtype == NBK_F4 || dtype == NBK_F8, "fft3pcf_gram: bad dtype %d", dtype);
-    NBK_CHECK_ARG(na >= 1 && na <= F3_MAX_SET && nb >= 1 && nb <= F3_MAX_SET, "fft3pcf_gram: %d x %d fields (1 .. %d each)",
+template <bool LIST>
+static int gram(const void *w, const void *A, int64_t a_stride, int na, const void *B, int64_t b_stride, int nb, int dtype,
+                int64_t ncell, const int64_t *tiles, int64_t ntiles, double *out, void *stream) {
+    const char *name = LIST ? "fft3pcf_gram_tiles" : "fft3pcf_gram";
+    NBK_CHECK_ARG(dtype == NBK_F4 || dtype == NBK_F8, "%s: bad dtype %d", name, dtype);
+    NBK_CHECK_ARG(na >= 1 && na <= F3_MAX_SET && nb >= 1 && nb <= F3_MAX_SET, "%s: %d x %d fields (1 .. %d each)", name,
                   na, nb, F3_MAX_SET);
     NBK_CHECK_ARG(ncell >= 0 && (na == 1 || a_stride >= ncell) && (nb == 1 || b_stride >= ncell),
-                  "fft3pcf_gram: bad field shape");
-    if (ncell == 0) return NBK_OK;
-    NBK_CHECK_ARG(w != nullptr && A != nullptr && B != nullptr && out != nullptr, "fft3pcf_gram: null pointer");
+                  "%s: bad field shape", name);
+    NBK_CHECK_ARG(!LIST || (ntiles >= 0 && ntiles <= (ncell + F3_TILE - 1) / F3_TILE), "%s: %lld tiles of %lld",
+                  name, (long long)ntiles, (long long)((ncell + F3_TILE - 1) / F3_TILE));
+    if (ncell == 0 || (LIST && ntiles == 0)) return NBK_OK;
+    NBK_CHECK_ARG(w != nullptr && A != nullptr && B != nullptr && out != nullptr && (!LIST || tiles != nullptr),
+                  "%s: null pointer", name);
     cudaStream_t s = (cudaStream_t)stream;
     const bool sym = A == B && na == nb && (na == 1 || a_stride == b_stride);
     if (dtype == NBK_F4) {
-        if (sym) return launch_gram<float, true>(w, A, a_stride, na, B, b_stride, nb, ncell, out, s);
-        return launch_gram<float, false>(w, A, a_stride, na, B, b_stride, nb, ncell, out, s);
+        if (sym) return launch_gram<float, true, LIST>(w, A, a_stride, na, B, b_stride, nb, ncell, tiles, ntiles, out, s);
+        return launch_gram<float, false, LIST>(w, A, a_stride, na, B, b_stride, nb, ncell, tiles, ntiles, out, s);
     }
-    if (sym) return launch_gram<double, true>(w, A, a_stride, na, B, b_stride, nb, ncell, out, s);
-    return launch_gram<double, false>(w, A, a_stride, na, B, b_stride, nb, ncell, out, s);
+    if (sym) return launch_gram<double, true, LIST>(w, A, a_stride, na, B, b_stride, nb, ncell, tiles, ntiles, out, s);
+    return launch_gram<double, false, LIST>(w, A, a_stride, na, B, b_stride, nb, ncell, tiles, ntiles, out, s);
+}
+
+extern "C" int nbk_fft3pcf_gram(const void *w, const void *A, int64_t a_stride, int na, const void *B, int64_t b_stride,
+                                int nb, int dtype, int64_t ncell, double *out, void *stream) {
+    return gram<false>(w, A, a_stride, na, B, b_stride, nb, dtype, ncell, nullptr, 0, out, stream);
+}
+
+extern "C" int nbk_fft3pcf_gram_tiles(const void *w, const void *A, int64_t a_stride, int na, const void *B,
+                                      int64_t b_stride, int nb, int dtype, int64_t ncell, const int64_t *tiles,
+                                      int64_t ntiles, double *out, void *stream) {
+    return gram<true>(w, A, a_stride, na, B, b_stride, nb, dtype, ncell, tiles, ntiles, out, stream);
 }
